@@ -6,7 +6,7 @@ benchmark generator), 64 Mi incoherent diffuse-bounce rays (33 cosine-weighted b
 image from inside the mesh, path-tracer style: tutorials/pathtracer/pathtracer_device.cpp:1119-1120,1597-1600), traced
 as batched rtcIntersect1 records.  A step = one pass of the 64 Mi-ray stream through the trace kernel.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--rays R] [--phi P]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--rays R] [--phi P] [--dump-outputs DIR]
 
 value  : Mrays/s with the RTCRayHit[] stream resident in HBM (rtcb200Intersect1MDevice on torch's current stream),
          whole job over all ranks (weak scaling: every rank traces its own 64 Mi rays; inside the timed region the
@@ -14,6 +14,9 @@ value  : Mrays/s with the RTCRayHit[] stream resident in HBM (rtcb200Intersect1M
 e2e    : the same stream through the host-pointer entry point rtcb200Intersect1M with pinned host buffers:
          H2D copy + trace + D2H copy inside the timed region.
 --impl reference : the unmodified reference (oracle/_ref/libembree4.so.4, else the C port) on the host cores.
+--dump-outputs DIR : after the timed steps, the hit records of the last timed step (a fixed, seeded sample of at most
+         1 Mi rays; --workload pathtracer: the radiance of as many paths) as DIR/<field>.npy, so that two builds can be
+         compared output for output on identical inputs.
 """
 import argparse
 import ctypes as C
@@ -43,7 +46,37 @@ def measured_peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         return json.load(open(p)), "measured (MEASURED_PEAKS.json hbm_gbs, burst copy)"
-    return {"hbm_gbs": 6650.0}, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return {"hbm_gbs": 3350.0}, "fallback (H100 SXM data sheet, 3.35 TB/s)"
+
+
+DUMP_SAMPLE = 1 << 20
+
+
+def dump_outputs(directory, records=None, extra=None):
+    """What the timed path returned in its last step, for output-by-output comparison of two builds on identical inputs:
+    the RTCRayHit fields a caller reads (float32; the ids as float64, which holds every uint32 exactly) of a fixed, seeded
+    sample of at most DUMP_SAMPLE records, ~50 MB.  A record without a hit (geomID 0xFFFFFFFF) keeps its input tfar, which
+    is +inf (or -inf for a path that has ended); it is written with tfar = -1 and Ng = u = v = 0, so that every value is
+    finite.  `extra`: further per-record outputs ({name: [n] tensor}), same sample; without `records` only those."""
+    os.makedirs(directory, exist_ok=True)
+    first = records if records is not None else next(iter(extra.values()))
+    n = first.shape[0]
+    idx = np.arange(n) if n <= DUMP_SAMPLE else np.sort(np.random.default_rng(0).choice(n, DUMP_SAMPLE, replace=False))
+    it = torch.from_numpy(idx).to(first.device)
+    out = {"ray_index": idx.astype(np.float64)}
+    if records is not None:
+        rec = records.index_select(0, it).cpu().numpy()
+        ids = rec.view(np.uint32)
+        miss = ids[:, 18] == 0xFFFFFFFF
+        rec[miss, 8] = -1.0
+        rec[miss, 12:17] = 0.0
+        out.update({"tfar": rec[:, 8], "Ng": rec[:, 12:15], "u": rec[:, 15], "v": rec[:, 16],
+                    "primID": ids[:, 17].astype(np.float64), "geomID": ids[:, 18].astype(np.float64)})
+    for k, x in (extra or {}).items():
+        out[k] = x.index_select(0, it).float().cpu().numpy()
+    for k, x in out.items():
+        np.save(os.path.join(directory, k + ".npy"), np.ascontiguousarray(x))
+    log(f"outputs of the last timed step: {len(idx)} of {n} records -> {directory}")
 
 
 def bounce_rays(primary_hits, ids, replicate=REPLICATE):
@@ -62,7 +95,7 @@ def bounce_rays(primary_hits, ids, replicate=REPLICATE):
 
 
 class ClockSampler(threading.Thread):
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
 
     def __init__(self, index):
         super().__init__(daemon=True)
@@ -120,7 +153,7 @@ def usable_cores():
 def bind_to_gpu_numa(local):
     """Multi-GPU runs: pin this rank (CPU affinity + memory policy) to the NUMA node its GPU hangs off, BEFORE any pinned
     host memory is allocated -- otherwise every rank's staging buffers land on the launching node and the ranks whose
-    GPUs sit on the other socket pull their rays across the inter-socket link (round 1: e2e scaled to 50 % at 8 GPUs)."""
+    GPUs sit on the other socket pull their rays across the inter-socket link."""
     info = {"node": None}
     try:
         pr = torch.cuda.get_device_properties(local)
@@ -220,7 +253,7 @@ def workload_config(args, ntris):
     return {"workload": f"configs[2]: createTriangleSphere(numPhi={args.phi}) = {ntris} triangles, BUILD_QUALITY_MEDIUM (device binned-SAH); "
                         f"{args.rays} incoherent diffuse-bounce rays ({REPLICATE} cosine-weighted bounces per hit of a {PRIMARY_W}x{PRIMARY_H} "
                         f"pinhole image from inside the mesh), batched rtcIntersect1 over RTCRayHit[]",
-            "rays_per_gpu": args.rays, "triangles": ntris, "l2": "ray stream 6.4 GB and BVH 0.6 GB per step exceed the 126 MB L2",
+            "rays_per_gpu": args.rays, "triangles": ntris, "l2": "ray stream 6.4 GB and BVH 0.6 GB per step exceed the 50 MB L2",
             "parallelism": f"ray-stream sharding x{args.gpus}, BVH replicated, compact hit records stored to rank 0 over NVLink by the trace kernel"}
 
 
@@ -650,7 +683,7 @@ def pathtracer_config(args, ntris, world):
                         f"(pathtracer_device.cpp:1489-1603): {args.rays} paths per GPU ({PRIMARY_W}x{PRIMARY_H} pinhole, jittered samples), "
                         f"{PT_BOUNCES} bounces, per bounce one batched rtcIntersect1 pass + one rtcOccluded1 shadow pass (matte material, one point light)",
             "paths_per_gpu": args.rays, "bounces": PT_BOUNCES, "rays_per_step_per_gpu": args.rays * PT_BOUNCES * 2, "triangles": ntris,
-            "l2": "each pass streams 3.2-6.4 GB of ray records: larger than the 126 MB L2",
+            "l2": "each pass streams 3.2-6.4 GB of ray records: larger than the 50 MB L2",
             "parallelism": f"path-stream sharding x{world}, BVH replicated, bounce generation local to each GPU, only the last bounce's compact "
                            "hit records are gathered to rank 0 (stored over NVLink by the trace kernel)"}
 
@@ -751,6 +784,8 @@ def run_pathtracer(args):
         dist.barrier()
     sampler.stop_flag = True
     launches = (lib.rtcb200GetLaunchCount() - l0) + args.steps * (1 + 2 * PT_BOUNCES)      # + primary / bounce / shade kernels
+    if args.dump_outputs and rank == 0:   # what the caller gets: the radiance per path (R already holds the next bounce's rays)
+        dump_outputs(args.dump_outputs, extra={"radiance": L})
     ms = torch.tensor([e0.elapsed_time(e1) / args.steps], device=devt)
     if world > 1:
         dist.all_reduce(ms, op=dist.ReduceOp.MAX)
@@ -918,6 +953,8 @@ def main():
     ap.add_argument("--no-e2e", action="store_true")
     ap.add_argument("--no-cpu", action="store_true")
     ap.add_argument("--no-extras", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's hit records (fixed seeded sample) as DIR/<field>.npy")
     ap.add_argument("--workload", default="diffuse", choices=["diffuse", "pathtracer"],
                     help="diffuse = configs[2] headline (default); pathtracer = configs[4] 8-bounce path stream")
     args = ap.parse_args()
@@ -988,9 +1025,7 @@ def main():
     # ---- hit gather (N > 1), fused into the trace kernel: rank 0 owns a [world, n, 8] float buffer, every rank maps it
     # through CUDA IPC and its trace kernel stores one compact 32-byte hit record per ray straight into its slice over
     # NVLink (rtcb200Intersect1MGatherDevice).  A tiny NCCL all-reduce, stream-ordered after the kernel, is the
-    # per-step "all hits have arrived" signal.  No separate collective moves hit data.  Measured: 99 % / 98 % of
-    # linear at 2 / 4 GPUs; at 8 GPUs the 15 GB per step that seven peers deliver into rank 0 take 86 ms (kernel alone:
-    # 50 ms): rank 0 ingests only ~175 GB/s (DESIGN.md section 7).
+    # per-step "all hits have arrived" signal.  No separate collective moves hit data (DESIGN.md section 7).
     gbuf, my_out, flag = None, None, None
     if world > 1:
         nbytes = world * n * 32
@@ -1039,6 +1074,8 @@ def main():
         dist.barrier()
     sampler.stop_flag = True
     launches = lib.rtcb200GetLaunchCount() - l0
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, B)
     ms_local = e0.elapsed_time(e1) / args.steps
     ms = torch.tensor([ms_local], device=devt)
     per_rank = None
@@ -1235,17 +1272,13 @@ def main():
         peaks, peak_src = measured_peaks()
         kms = float(np.mean(kernel_ms)) if kernel_ms else ms_per_step
         achieved = bytes_per_ray * n / (kms * 1e-3) * 1e-9
-        traffic = None
-        tp = os.path.join(ROOT, "profiles", "ncu_traffic.json")
-        if os.path.exists(tp):
-            traffic = json.load(open(tp)).get("dram_bytes_per_launch")
         line = {"metric": "Mrays/s incoherent diffuse-bounce, 10M-triangle scene", "value": value, "unit": "Mrays/s", "n_gpus": world,
                 "steps": args.steps, "warmup": args.warmup, "ms_per_step": ms_per_step, "higher_is_better": True, "scaling": "weak",
                 "vs_baseline": None, "dtype": "f32", "data": "synthetic", "config": workload_config(args, len(t)),
                 "clocks": sampler.summary(), "e2e": e2e, "gpu_launches": int(launches), "gather_verified": gather_ok, "per_rank": per_rank,
                 "gather_ab": gather_ab, "numa": numa,
                 "roofline": {"bound": "hbm", "achieved": achieved, "peak": peaks["hbm_gbs"], "unit": "GB/s", "frac": achieved / peaks["hbm_gbs"],
-                             "traffic": traffic, "peak_source": peak_src,
+                             "traffic": None, "peak_source": peak_src,
                              "kernel": "rtk::trace_kernel<K=1,OCCLUDED=false,STATS=false,ROBUST=false,GENERAL=0,GATHER=0,SPREAD=true>",
                              "kernel_ms": kms, "algorithmic_bytes_per_ray": bytes_per_ray,
                              "frac_with_round1_80B_nodes": (100 + nodes_per_ray * 80 + tris_per_ray * 48) * n / (kms * 1e-3) * 1e-9 / peaks["hbm_gbs"],

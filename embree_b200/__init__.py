@@ -1,6 +1,6 @@
-"""embree_b200 -- B200-native ray tracing kernels behind the Embree 4 C API.
+"""embree_b200 -- H100-native ray tracing kernels behind the Embree 4 C API.
 
-The product is the C-ABI shared library embree_b200/csrc/libembree4_b200.so (hand-written sm_100a CUDA +
+The product is the C-ABI shared library embree_b200/csrc/libembree4_b200.so (hand-written sm_90a CUDA +
 the C++ host shim); this package only locates/loads it for the Python tests and bench.py.  There is no CPU or
 PyTorch fallback: if the library has not been built (python __graft_entry__.py / make -C embree_b200/csrc),
 `load()` raises.
@@ -22,7 +22,7 @@ def load():
         if not os.path.exists(LIB_PATH):
             raise RuntimeError(
                 f"{LIB_PATH} is missing: build it with `python -c 'import __graft_entry__ as g; g.build()'` "
-                "(nvcc, sm_100a).  embree_b200 has no CPU fallback.")
+                "(nvcc, sm_90a).  embree_b200 has no CPU fallback.")
         _lib = RTCLib(LIB_PATH)
         if not _lib.is_b200:
             raise RuntimeError(f"{LIB_PATH} does not export the rtcb200* entry points")

@@ -1,4 +1,4 @@
-// build.cu -- device-wide BVH construction for sm_100a.
+// build.cu -- device-wide BVH construction for sm_90a.
 //
 // Replaces (reference paths): kernels/builders/primrefgen.cpp:14-60 + scene_triangle_mesh.h:194-215,293-305
 // (PrimRef generation with the validity filter), kernels/builders/bvh_builder_morton.h:71-102,312-432
@@ -706,7 +706,7 @@ int build_sah_tree(const PrimRef* prims, uint32_t* idsA, uint32_t* idsB, uint32_
 // ---------------------------------------------------------------------------------------------------
 // Build temporaries come from the device's stream-ordered memory pool (cudaMallocAsync): after the first commit the
 // pool serves every later build without touching the driver allocator, which is what keeps per-frame rebuilds of
-// dynamic scenes at kernel time (a plain cudaMalloc/cudaFree pair per buffer cost 10-300 ms at 10 M triangles).
+// dynamic scenes at kernel time (a plain cudaMalloc/cudaFree pair per buffer is slow at 10 M triangles).
 // The pool is the device's default one, which other users of cudaMallocAsync in the process share: the amount it may keep
 // cached after a commit is bounded (device config key "pool_keep_mb", default 8192 MB -- enough for the temporaries of a
 // 10 M-triangle build; memory above that goes back to the driver at the next synchronisation).

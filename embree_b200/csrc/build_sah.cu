@@ -653,7 +653,7 @@ int build_sah_tree(const PrimRef* prims, uint32_t* idsA, uint32_t* idsB, uint32_
   const size_t smem_block = sizeof(GroupSmem) + (size_t)kBlockCap * 8;
   const size_t smem_warp = (sizeof(GroupSmem) + (size_t)kWarpCap * 8) * WARP_GROUPS;
   CKC(cudaFuncSetAttribute(sah_group_kernel<BLOCK_NT, 1, kBlockCap>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_block));
-  int sms = 148;
+  int sms = 132;
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, 0);
 
   int cur = 0;

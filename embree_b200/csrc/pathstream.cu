@@ -1,7 +1,7 @@
 // pathstream.cu -- wavefront form of the reference's path-tracer tile loop, the CALLER of the hot path for BASELINE
 // configs[4] (tutorials/pathtracer/pathtracer_device.cpp:1489-1603): one stream of RTCRayHit records per GPU, and per
 // bounce   rtcb200Intersect1MDevice -> pts200_bounce -> rtcb200Occluded1MDevice -> pts200_shade.
-// The kernels here are hand-written sm_100a CUDA in their own small C-ABI library (libpathstream_b200.so): they are
+// The kernels here are hand-written sm_90a CUDA in their own small C-ABI library (libpathstream_b200.so): they are
 // tutorial-side code, not part of the Embree API, and link nothing from libembree4_b200.so.
 //
 // What one reference loop iteration does after rtcIntersect1, restated per path (thread = path, records in place):

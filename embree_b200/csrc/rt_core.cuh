@@ -1,4 +1,4 @@
-// rt_core.cuh -- data layout and per-ray / per-node core routines of the B200 ray tracing kernels.
+// rt_core.cuh -- data layout and per-ray / per-node core routines of the CUDA ray tracing kernels.
 //
 // Everything here is `RT_HD` (__host__ __device__) on purpose: the CUDA kernels in build.cu / trace.cu call
 // these routines per thread, and tests/emu/ compiles the very same header with g++ so the node encoding,
@@ -28,8 +28,8 @@ namespace rtk {
 // ------------------------------------------------------------------------------------------------
 // HBM layout
 // ------------------------------------------------------------------------------------------------
-// BVH8 node, 96 bytes = 3 x 32 B, 32-byte aligned: one node is three 256-bit loads (LDG.E.256 on sm_100a), each a
-// whole DRAM/L2 sector (compressed wide BVH: 8-bit child boxes on a per-node power-of-two grid).
+// BVH8 node, 96 bytes = 3 x 32 B, 32-byte aligned: one node is three whole DRAM/L2 sectors (compressed wide BVH:
+// 8-bit child boxes on a per-node power-of-two grid).
 //   w0..w2  : px, py, pz (float bits) -- origin of the node's grid
 //   w3      : ex | ey<<8 | ez<<16 | imask<<24   (biased exponents of the grid scale per axis; imask bit s = slot s
 //             holds an internal child)
@@ -1257,7 +1257,7 @@ RT_HD void collapse_node(const Node2* n2, uint32_t* src, uint32_t q, Node8* n8, 
 // pointers and the device can use the read-only / cache-hinted path.
 // ------------------------------------------------------------------------------------------------
 struct u32x4 { uint32_t x, y, z, w; };
-struct NodeW { uint32_t w[24]; };   // one node in registers (three 256-bit loads)
+struct NodeW { uint32_t w[24]; };   // one node in registers (three 32-byte sectors)
 struct TravStats { uint32_t nodes, tris; };
 
 // Slab test of the 8 quantised children of one node; returns the hit mask in the layout
@@ -1285,8 +1285,6 @@ RT_HD uint32_t node_hitmask(const uint32_t* w, float ox, float oy, float oz, flo
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
       const int sh = 8 * j;
-      // (packed fp32 FMAs -- fma.rn.f32x2 / FFMA2 on sm_100a, two children per instruction -- were measured 3-8 % SLOWER:
-      // the aligned register pairs they need add spills in this loop, profiles/r2_ab_runs.txt run 10)
       const float tnx = fma_rn((float)((nx >> sh) & 0xFFu), sx, bx);
       const float tny = fma_rn((float)((ny >> sh) & 0xFFu), sy, by);
       const float tnz = fma_rn((float)((nz >> sh) & 0xFFu), sz, bz);

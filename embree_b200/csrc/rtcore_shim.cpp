@@ -496,10 +496,9 @@ void commit_scene(SceneImpl* s) {
     for (GeometryImpl* g : geoms) if (g && g->enabled) { plain = plain && g->type == RTC_GEOMETRY_TYPE_TRIANGLE; ++ntri_geoms; }
     bool eligible = plain && ntri_geoms >= 2 && (s->flags & RTC_SCENE_FLAG_DYNAMIC) && !getenv("RTCB200_NO_TWOLEVEL");
     if (eligible && !getenv("RTCB200_FORCE_TWOLEVEL")) {
-      // Which regime is cheaper for THIS commit?  A device build runs at ~400 Mprims/s plus ~0.5 ms of launches and round trips per
-      // build, the vertex upload at PCIe speed: rebuilding one BVH over everything costs ~1.5 ms + 2.5 ns per triangle, the two-level
-      // commit ~1 ms + (0.5 ms + 2.5 ns per triangle) per mesh modified since the last commit (measured, bench.py
-      // extras.dynamic_scene_two_level).  When most meshes move every frame (tutorials/dynamic_scene) one rebuild wins; when a few of
+      // Which regime is cheaper for THIS commit?  Cost model: rebuilding one BVH over everything costs ~1.5 ms + 2.5 ns per
+      // triangle (device build plus the vertex upload at PCIe speed), the two-level commit ~1 ms + (0.5 ms + 2.5 ns per triangle)
+      // per mesh modified since the last commit (bench.py extras.dynamic_scene_two_level times both paths).  When most meshes move every frame (tutorials/dynamic_scene) one rebuild wins; when a few of
       // many move, the two-level path does -- meshes that have no kept BVH yet are built then, a one-time investment.
       double total = 0.0, two = 1.0;
       for (size_t id = 0; id < geoms.size(); ++id) {
@@ -632,7 +631,9 @@ void commit_scene(SceneImpl* s) {
       }
   }
   s->gpu.general = (instanced || quads || curves) ? 1 : 0;
-  s->gpu.curves = curves ? 1 : 0;
+  // 2: curve records among them, 1: point records only -- the two kinds take different leaf-test batching and grid (rtk::Tuning)
+  const bool curve_records = std::any_of(descs.begin(), descs.end(), [](const rtk::GeomDesc& d) { return d.is_curve >= 1 && d.is_curve <= 4; });
+  s->gpu.curves = curves ? (curve_records ? 2 : 1) : 0;
   // quality -> builder (scene.cpp:163-206: LOW = Morton two-level builder, MEDIUM/HIGH = SAH).  The env override
   // exists for A/B measurements of the two device builders only.
   rtk::BuilderKind kind = (s->quality == RTC_BUILD_QUALITY_LOW) ? rtk::BUILDER_LBVH : rtk::BUILDER_SAH;
@@ -804,12 +805,11 @@ void trace_device(SceneImpl* s, void* d_rays, const int* d_valid, int K, size_t 
 // `compact_out` -- local memory or a peer's memory over NVLink -- so the transfer is spread over the whole launch and no
 // separate collective moves hit data.  rtcb200SetTuning("gather_mode", m): 1 (default) writes each record to a local staging
 // buffer first and sends complete 32-ray blocks as 1 KB (eight full lines); 0 stores every record on its own as
-// one 256-bit sector when its ray terminates (round 1: 99 % / 98 % of linear at 2 / 4 GPUs but only ~225 GB/s into
-// rank 0 at 8 GPUs).  The copy-engine pipeline round 1 carried as an unvalidated option is gone.
+// one 32-byte sector when its ray terminates (with many peers, rank 0's ingest of single sectors is request-rate bound).
 void trace_gather(SceneImpl* s, void* d_rays, size_t M, uint32_t instID, uint32_t instPrimID, cudaStream_t st, void* compact_out) {
   require_committed(s);
   if (M == 0) return;
-  if (reinterpret_cast<uintptr_t>(compact_out) & 31) fail(RTC_ERROR_INVALID_ARGUMENT, "compact_out must be 32-byte aligned (one 256-bit store per record)");
+  if (reinterpret_cast<uintptr_t>(compact_out) & 31) fail(RTC_ERROR_INVALID_ARGUMENT, "compact_out must be 32-byte aligned (one sector per record)");
   cudaSetDevice(s->dev->gpu);
   if (!s->ev0) { cudaEventCreate(&s->ev0); cudaEventCreate(&s->ev1); }
   cudaEventRecord(s->ev0, st);
@@ -831,12 +831,11 @@ void trace_gather(SceneImpl* s, void* d_rays, size_t M, uint32_t instID, uint32_
 
 // batched, host pointers: chunked H2D -> trace -> D2H pipeline over three streams
 // host-buffer pipeline shape (rtcb200SetTuning "host_chunk_log2" / "host_streams"): rays per chunk and chunks in flight
-static int g_host_chunk_log2 = 20, g_host_streams = 3;   // measured: 2^20 -> 492 Mrays/s, 2^22 -> 474 (scripts/e2e_sweep.py)
+static int g_host_chunk_log2 = 20, g_host_streams = 3;   // scripts/e2e_sweep.py sweeps both
 // rtcb200SetTuning("host_d2h_partial", 1): the copy back to the host skips the bytes of a record that a query never changes -- org, tnear,
 // dir, time of an RTCRayHit (the first 32 of its 96 bytes), the first eight fields of an RTCRayHitK -- with a pitched copy of the rest.
-// Fewer bytes cross PCIe and, with several GPUs per socket, the host's memory controllers (the limit of the 8-GPU e2e number) -- but the
-// copy engine moves 64-byte rows of a pitched copy slower than one contiguous block: measured at one GPU 431 vs 490 Mrays/s
-// (scripts/e2e_partial_ab.py, identical records), so it is OFF by default; not measured at 8 GPUs.
+// Fewer bytes cross PCIe and, with several GPUs per socket, the host's memory controllers -- but the copy engine moves the 64-byte
+// rows of a pitched copy slower than one contiguous block (scripts/e2e_partial_ab.py compares both), so it is OFF by default.
 static int g_host_d2h_partial = 0;
 
 struct HostPipe {
@@ -1123,13 +1122,13 @@ RTCDevice rtcNewDevice(const char* config) {
   cudaGetDeviceCount(&count);
   if (d->gpu < 0 || d->gpu >= count) { delete d; d = nullptr; fail(RTC_ERROR_INVALID_ARGUMENT, "gpu ordinal out of range"); }
   cuda_check(cudaGetDeviceProperties(&d->prop, d->gpu), "cudaGetDeviceProperties");
-  if (d->prop.major < 10) {
-    std::string m = std::string("this library contains sm_100a code only; device is ") + d->prop.name;
+  if (d->prop.major != 9 || d->prop.minor != 0) {
+    std::string m = std::string("this library contains sm_90a code only; device is ") + d->prop.name;
     delete d; d = nullptr;
     fail(RTC_ERROR_UNKNOWN, m.c_str());
   }
   if (d->verbose >= 1)
-    fprintf(stderr, "Embree-API B200 kernels %s: GPU %d %s, %d SMs, %.0f GB\n", RTC_VERSION_STRING, d->gpu, d->prop.name,
+    fprintf(stderr, "Embree-API CUDA kernels %s: GPU %d %s, %d SMs, %.0f GB\n", RTC_VERSION_STRING, d->gpu, d->prop.name,
             d->prop.multiProcessorCount, d->prop.totalGlobalMem / 1e9);
   return reinterpret_cast<RTCDevice>(d);
   API_END(nullptr)
@@ -1204,7 +1203,7 @@ RTCGeometry rtcNewGeometry(RTCDevice h, enum RTCGeometryType type) {
   API_BEGIN
   VERIFY_HANDLE(h);
   if (type != RTC_GEOMETRY_TYPE_TRIANGLE && type != RTC_GEOMETRY_TYPE_QUAD && type != RTC_GEOMETRY_TYPE_INSTANCE && !is_linear_curve(type) && !is_cubic_curve(type) && !is_point(type))
-    fail(RTC_ERROR_INVALID_OPERATION, "only RTC_GEOMETRY_TYPE_TRIANGLE, _QUAD, _ROUND / _FLAT_LINEAR_CURVE, _ROUND / _FLAT_BEZIER / _BSPLINE / _HERMITE / _CATMULL_ROM_CURVE, _SPHERE / _DISC / _ORIENTED_DISC_POINT and _INSTANCE are supported by the B200 back-end");
+    fail(RTC_ERROR_INVALID_OPERATION, "only RTC_GEOMETRY_TYPE_TRIANGLE, _QUAD, _ROUND / _FLAT_LINEAR_CURVE, _ROUND / _FLAT_BEZIER / _BSPLINE / _HERMITE / _CATMULL_ROM_CURVE, _SPHERE / _DISC / _ORIENTED_DISC_POINT and _INSTANCE are supported by the CUDA back-end");
   GeometryImpl* g = new GeometryImpl(D(h));
   g->type = type;
   return reinterpret_cast<RTCGeometry>(g);
@@ -1293,7 +1292,7 @@ void rtcSetGeometryTessellationRate(RTCGeometry g, float n) {
   G(g)->update();
   GEOM_END
 }
-void rtcSetGeometryTimeStepCount(RTCGeometry g, unsigned int n) { GEOM_BEGIN(g) if (n != 1) fail(RTC_ERROR_INVALID_OPERATION, "motion blur is not supported by the B200 back-end"); GEOM_END }
+void rtcSetGeometryTimeStepCount(RTCGeometry g, unsigned int n) { GEOM_BEGIN(g) if (n != 1) fail(RTC_ERROR_INVALID_OPERATION, "motion blur is not supported by the CUDA back-end"); GEOM_END }
 void rtcSetGeometryVertexAttributeCount(RTCGeometry g, unsigned int n) { GEOM_BEGIN(g) G(g)->attribs.resize(n); G(g)->update(); GEOM_END }
 void rtcSetGeometryMask(RTCGeometry g, unsigned int mask) { GEOM_BEGIN(g) G(g)->mask = mask; G(g)->update(); GEOM_END }
 void rtcSetGeometryBuildQuality(RTCGeometry g, enum RTCBuildQuality q) {
@@ -1627,6 +1626,9 @@ int rtcb200SetTuning(const char* key, int value) {
   else if (!strcmp(key, "curve_batch_min")) t.curve_batch_min = value;
   else if (!strcmp(key, "curve_wait_max")) t.curve_wait_max = value;
   else if (!strcmp(key, "blocks_per_sm")) t.blocks_per_sm = value;
+  else if (!strcmp(key, "curve_blocks_per_sm")) t.curve_blocks_per_sm = value;
+  else if (!strcmp(key, "point_batch_min")) t.point_batch_min = value;
+  else if (!strcmp(key, "point_wait_max")) t.point_wait_max = value;
   else if (!strcmp(key, "use_tma")) t.use_tma = value;
   else if (!strcmp(key, "tri_spread")) t.tri_spread = value != 0;
   else if (!strcmp(key, "tri_spread_occluded")) t.tri_spread_occluded = value != 0;
@@ -1726,7 +1728,7 @@ void rtcSetGeometryMaxRadiusScale(RTCGeometry g, float) { GEOM_BEGIN(g) G(g)->up
 // RTC_ERROR_INVALID_OPERATION (thread error slot, read with rtcGetDeviceError(NULL)) and returns 0 / NULL / false.
 #define RTCB200_UNSUPPORTED(name)                                                                              \
   void* name(void) {                                                                                           \
-    process_error(nullptr, RTC_ERROR_INVALID_OPERATION, #name " is not supported by the B200 triangle back-end"); \
+    process_error(nullptr, RTC_ERROR_INVALID_OPERATION, #name " is not supported by the CUDA triangle back-end"); \
     return nullptr;                                                                                            \
   }
 RTCB200_UNSUPPORTED(rtcBuildBVH)

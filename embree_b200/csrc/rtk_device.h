@@ -78,7 +78,7 @@ struct SceneGPU {
   uint32_t root_valid = 0;              // 0: empty scene -> queries return immediately
   int robust = 0;                       // RTC_SCENE_FLAG_ROBUST: leaf records are (v0, v1, v2), Pluecker intersector
   int general = 0;                      // scene has instances, quads or curves: records carry a descriptor index instead of geomID
-  int curves = 0;                       // scene has round linear curve records
+  int curves = 0;                       // scene has curve or point records: 2 curve records among them, 1 point records only
   GeomDesc* d_descs = nullptr;          // device copy of the mesh descriptors (kept while general)
   float bounds[6] = {0, 0, 0, 0, 0, 0};  // lower xyz, upper xyz of all valid triangles (world space, instances flattened)
   float api_bounds[6] = {0, 0, 0, 0, 0, 0};  // the same without instanced triangles
@@ -129,7 +129,7 @@ struct TraceParams {
   void* stage = nullptr;   // gather mode 1: local staging buffer with the same indexing (n x 32 B)
   int tri_batch_min = 8, tri_wait_max = 4, refill_min = 4, use_prefetch = 1;  // filled by launch_trace from tuning()
   const GeomDesc* descs = nullptr;  // non-NULL: instanced scene, record.geomID slot holds a descriptor index
-  int curves = 0;                   // the scene holds round linear curve records (descs != NULL)
+  int curves = 0;                   // the scene holds curve or point records (descs != NULL): 2 curves among them, 1 points only
   uint32_t top_nodes = 0;           // nodes in the first three BVH8 levels (RTK_TOP_SMEM experiment)
   int robust = 0;  // scene built with RTC_SCENE_FLAG_ROBUST: triangle records hold v0,v1,v2, Pluecker test
   // filter-callback passes (K == 1 closest hit): per-ray lists of rejected record indices (excl_off has n + 1 entries) and
@@ -148,12 +148,15 @@ struct Tuning {
   int tri_batch_min = 8;     // triangle step when >= this many lanes have triangles pending (or no lane has a node, or after tri_wait_max deferrals)
   int tri_wait_max = 4;
   // the same two keys for scenes with curve records: a curve test costs 10-100x a triangle test, so it pays to wait until more
-  // lanes have one pending (measured on the fur ball of bench.py: flat +13 / +20 %, round +43 / +56 % over 8 / 4; scripts/hair_tune.py)
-  int curve_batch_min = 24, curve_wait_max = 16;
+  // lanes have one pending (scripts/hair_tune.py sweeps both on the fur ball of bench.py); scenes of points only take their own
+  // pair.  Curve scenes also run with fewer CTAs per SM (curve_blocks_per_sm).
+  int curve_batch_min = 32, curve_wait_max = 24;
+  int point_batch_min = 24, point_wait_max = 16;
   int blocks_per_sm = 8;
+  int curve_blocks_per_sm = 6;
   int use_tma = 1;
   int refill_min = 4;
-  int gather_mode = 1;       // fused hit gather: 0 = one 256-bit store per record, 1 = blocks staged in shared memory, 1 KB stores
+  int gather_mode = 1;       // fused hit gather: 0 = one 32-byte store per record, 1 = blocks staged in shared memory, 1 KB stores
   int tri_spread = 1;        // warp-wide triangle redistribution in the trace kernel (trace.cu SPREAD; closest-hit triangle scenes)
   int tri_spread_occluded = 1;   // the same redistribution in the any-hit kernels (a hit ends the owner's ray)
   int sah_small = 4;         // SAH builder: segments of <= this many primitives are split in the middle (no binning)

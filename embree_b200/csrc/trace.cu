@@ -1,4 +1,4 @@
-// trace.cu -- closest-hit / any-hit traversal kernels for sm_100a.
+// trace.cu -- closest-hit / any-hit traversal kernels for sm_90a.
 //
 // Replaces kernels/bvh/bvh_intersector1.cpp:31-197 (single ray) and, through the packet I/O adapters below,
 // kernels/bvh/bvh_intersector_hybrid.cpp:106-370,600-783 (rtcIntersect4/8/16, rtcOccluded4/8/16): on this
@@ -11,11 +11,11 @@
 namespace rtk {
 
 // ---- loads of the BVH through the read-only path -----------------------------------------------------------------
-// A node is 96 bytes, 32-byte aligned: three 256-bit loads (ld.global.nc.v8.b32 -> LDG.E.ENL2.256.CONSTANT on sm_100a),
-// each exactly one sector.  Round 1 fetched an 80-byte node with five 16-byte loads: 5 L1 tag lookups per lane per node
-// instead of 3, and the same three sectors from L2 / HBM.
+// A node is 96 bytes, 32-byte aligned: three sectors.  sm_90 has no 256-bit load, so each sector is two 128-bit
+// read-only loads (ld.global.nc.v4.b32 -> LDG.E.128.CONSTANT) issued back to back; both halves hit the same sector.
 __device__ __forceinline__ void ldg256(const void* p, uint32_t* d) {
-  asm volatile("ld.global.nc.v8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
+  asm volatile("ld.global.nc.v4.b32 {%0,%1,%2,%3}, [%8];\n\t"
+               "ld.global.nc.v4.b32 {%4,%5,%6,%7}, [%8+16];"
                : "=r"(d[0]), "=r"(d[1]), "=r"(d[2]), "=r"(d[3]), "=r"(d[4]), "=r"(d[5]), "=r"(d[6]), "=r"(d[7])
                : "l"(p));
 }
@@ -141,9 +141,10 @@ __device__ __noinline__ bool curve_record_test(const GeomDesc& d, const Ray& r, 
   return curve_test(r.ox, r.oy, r.oz, r.dx, r.dy, r.dz, r.tnear, tfar, v0, v1, hasL, vL, hasR, vR, h);
 }
 
-// 32-byte aligned 256-bit global store (PTX st.global.v8.f32 -> STG.E.256 on sm_100a)
+// one 32-byte aligned sector written as two 128-bit global stores (sm_90 has no 256-bit store)
 __device__ __forceinline__ void store_256(void* dst, float a0, float a1, float a2, float a3, float a4, float a5, float a6, float a7) {
-  asm volatile("st.global.v8.f32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};" ::"l"(dst), "f"(a0), "f"(a1), "f"(a2), "f"(a3), "f"(a4),
+  asm volatile("st.global.v4.f32 [%0], {%1, %2, %3, %4};\n\t"
+               "st.global.v4.f32 [%0+16], {%5, %6, %7, %8};" ::"l"(dst), "f"(a0), "f"(a1), "f"(a2), "f"(a3), "f"(a4),
                "f"(a5), "f"(a6), "f"(a7)
                : "memory");
 }
@@ -152,8 +153,8 @@ constexpr int TRACE_THREADS = 128;
 constexpr int TRACE_WARPS = TRACE_THREADS / 32;
 
 // ---- TMA bulk prefetch of one 32-ray block (1.5 .. 3 KB contiguous) into L2 ------------------------------------------
-// Staging the blocks in shared memory (cp.async.bulk.shared + mbarrier) was measured SLOWER (1012 vs 1380 Mrays/s):
-// 24 KB of shared memory per CTA x 8 CTAs/SM leaves only ~30 KB of L1, and the BVH lives on L1 hits.  The bulk
+// Staging the blocks in shared memory (cp.async.bulk.shared + mbarrier) instead would take 24 KB of shared memory per
+// CTA x 8 CTAs/SM out of the 256 KB an SM shares between L1 and shared memory, and the BVH lives on L1 hits.  The bulk
 // prefetch keeps the TMA unit pulling the ray stream ahead of the warps without costing L1 capacity.
 __device__ __forceinline__ void tma_prefetch_l2(const void* src, uint32_t bytes) {
   asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(src), "r"(bytes) : "memory");
@@ -168,7 +169,7 @@ __device__ __forceinline__ void tma_prefetch_l2(const void* src, uint32_t bytes)
 #endif
 #ifndef RTK_TOP_SMEM
 #define RTK_TOP_SMEM 0     // EXPERIMENT: this many nodes from the top of the (breadth-first) node array are staged in shared memory
-#endif                     // with one TMA bulk copy per CTA (cp.async.bulk + mbarrier); 73 = root + 8 + 64.  Measured: see DESIGN.md
+#endif                     // with one TMA bulk copy per CTA (cp.async.bulk + mbarrier); 73 = root + 8 + 64
 #ifndef RTK_LANE_SMEM
 #define RTK_LANE_SMEM 1    // per-lane state that only the hit update and the write-back touch (u, v, winning record, ray index)
 #endif                     // lives in shared memory instead of registers
@@ -190,20 +191,19 @@ __device__ __forceinline__ void tma_prefetch_l2(const void* src, uint32_t bytes)
 //   3. at most one triangle step, batched across the warp;
 //   4. pop.  The top stack entry lives in registers as a write-back cache of the local-memory stack: a pop that
 //      follows a push costs no memory access, and a local-memory load is only waited for when two pops follow each
-//      other (round 1 reloaded the register copy on every pop and stalled on it: 7.5 % of all issue-stall samples).
+//      other (reloading the register copy on every pop stalls on the local-memory load).
 // The phases are warp-synchronous so lanes in the same phase execute together instead of serialising through a
 // per-thread while-while loop.
 //
 // GATHER (K == 1 closest hit only) adds the fused multi-GPU hit gather: every ray also produces one compact 32-byte
 // record {tfar, Ng, u, v, primID, geomID} in `compact_out`, which may be a PEER GPU's memory (NVLink).
-//   GATHER 1: the lane stores its record when the ray is written back -- one 256-bit store (STG.E.256), one sector.
+//   GATHER 1: the lane stores its record when the ray is written back -- one sector (two 128-bit stores).
 //   GATHER 2: records are first stored to a LOCAL staging buffer (p.stage, same indexing); the warp tracks which records of
 //             its two newest 32-ray blocks have arrived and, when a block is complete, re-reads its 1 KB (L2 hits) and sends
-//             it as ONE warp-wide store of eight full 128-byte lines.  At 8 GPUs seven peers store into rank 0; with
-//             single-sector stores rank 0 ingested only ~225 GB/s (request-rate bound), which held the 8-GPU step at 67 ms
-//             instead of 50 ms.  A block that stops being tracked before all its rays have finished is sent partially
-//             (masked lanes) and its stragglers fall back to the direct store.  (Staging in shared memory -- two 1 KB slots
-//             per warp -- cost 20 % of the kernel at 2 GPUs, profiles/r2_bench_n2.json gather_ab: 8 KB less L1 per CTA.)
+//             it as ONE warp-wide store of eight full 128-byte lines.  With several peers storing into rank 0, single-sector
+//             stores make rank 0's ingest request-rate bound.  A block that stops being tracked before all its rays have
+//             finished is sent partially (masked lanes) and its stragglers fall back to the direct store.  (The staging
+//             buffer is in global memory: two 1 KB slots per warp in shared memory would take 8 KB of L1 per CTA.)
 //
 // FILTER (K == 1 closest hit, host-pointer entry points only): the host side of filter callbacks (rtcore_shim.cpp
 // trace_filtered).  Every ray carries a list of record indices that a callback has already rejected
@@ -253,7 +253,7 @@ __global__ void __launch_bounds__(TRACE_THREADS, RTK_MIN_BLOCKS) trace_kernel(co
   float hit_u = 0, hit_v = 0;
   uint32_t hit_tri = 0;
   uint32_t ray_index = 0;
-#error "RTK_LANE_SMEM=0 is no longer supported (kept only in the history of profiles/r2_ab_runs.txt)"
+#error "RTK_LANE_SMEM=0 is no longer supported"
 #endif
   // this lane's ray with the parked fields filled in (non-SPREAD triangle / curve tests, ROBUST write-back)
   auto full_ray = [&]() -> Ray {
@@ -266,9 +266,8 @@ __global__ void __launch_bounds__(TRACE_THREADS, RTK_MIN_BLOCKS) trace_kernel(co
   uint32_t ngx = 0, ngy = 0, tgx = 0, tgy = 0;
   uint32_t top_x = 0, top_y = 0;          // register copy of the newest stack entry (top_y == 0: none)
   // older entries: the first RTK_SMEM_STACK per lane in shared memory ([entry][thread]: conflict-free 8-byte accesses),
-  // deeper ones in local memory.  Round 1 kept the whole stack in local memory: its lines compete with the streaming
-  // node / triangle data for L1, a pop that missed cost an L2 round trip (~500 cycles, 7 % of all stall samples) and
-  // every push was written through to L2 (26 GB per 64 Mi-ray launch).
+  // deeper ones in local memory.  A stack wholly in local memory competes with the streaming node / triangle data for L1,
+  // a pop that misses costs an L2 round trip, and every push is written through to L2.
   __shared__ uint2 s_stack[RTK_SMEM_STACK > 0 ? RTK_SMEM_STACK * TRACE_THREADS : 1];
   uint2 stack[kStackSize];
   int sp = 0;
@@ -290,8 +289,8 @@ __global__ void __launch_bounds__(TRACE_THREADS, RTK_MIN_BLOCKS) trace_kernel(co
   // GATHER 2: the two newest blocks of this warp are tracked; slot_blk = index (in this warp's block sequence), slot_have =
   // which of its 32 records have been written to the local staging buffer (warp-uniform values)
   // The state lives in shared memory (16 B per warp: first ray index and arrival mask of the two tracked blocks), not in
-  // registers: it is only touched in the write-back phase, and four more live registers in the traversal loop cost 19 % of
-  // the kernel (first version of this mode, r2_bench_n2_smem_staging.json).
+  // registers: it is only touched in the write-back phase, and four more live registers in the traversal loop spill in the
+  // node step.
   __shared__ uint32_t s_slot[GATHER == 2 ? TRACE_WARPS : 1][4];   // first0, have0, first1, have1; first == ~0u: free
   constexpr uint32_t kNoBlock = 0xFFFFFFFFu;
   if (GATHER == 2) {
@@ -382,7 +381,7 @@ __global__ void __launch_bounds__(TRACE_THREADS, RTK_MIN_BLOCKS) trace_kernel(co
       }
     }
     if (FILTER) p.win[ray_index] = found ? hit_tri : kInvalidID;
-    if (GATHER)   // one 256-bit store (STG.256, new on sm_100): a full 32-byte sector; a miss (also: empty scene) yields {tfar, 0.., -1, -1}
+    if (GATHER)   // a full 32-byte sector; a miss (also: empty scene) yields {tfar, 0.., -1, -1}
       store_256(rec_dst, tfar_tri, cngx, cngy, cngz, found ? hit_u : 0.0f, found ? hit_v : 0.0f, __uint_as_float(cprim), __uint_as_float(cgeom));
   };
   // GATHER 2: send the arrived records of a tracked block from the staging buffer to the gather buffer, lane i = record i
@@ -466,7 +465,7 @@ __global__ void __launch_bounds__(TRACE_THREADS, RTK_MIN_BLOCKS) trace_kernel(co
     const unsigned idle = __ballot_sync(FULL, state != TRACING);
     if (idle && (__popc(idle) >= refill_min || idle == FULL)) {
       // (Issuing the record fetches of the write-back together with the ray fetches of the refill -- one latency instead
-      // of two -- was measured 10 % SLOWER, profiles/r2_ab_runs.txt run 3: the extra live registers spill in the node step.)
+      // of two -- is not done: the extra live registers spill in the node step.)
       const bool has_rec = state == DONE;
       int slot = -1;
       uint32_t first0 = 0, first1 = 0;
@@ -602,8 +601,8 @@ __global__ void __launch_bounds__(TRACE_THREADS, RTK_MIN_BLOCKS) trace_kernel(co
       if (SPREAD) {
         // Closest-hit Moeller-Trumbore triangle scenes (rtcb200SetTuning "tri_spread" 0 turns it off): the pending
         // triangles of ALL lanes become work items that the whole warp tests in one step, instead of each lane testing
-        // one of its own while the others idle.  Measured on the headline stream: 12.6 triangle steps per 32 rays with
-        // 19 lanes busy instead of 27 steps with 9, +11 % Mrays/s (profiles/r2_ab_runs.txt).  Owners queue (record index, owner lane) in shared memory; worker lane w takes item w, fetches the
+        // one of its own while the others idle: on the headline stream about half as many triangle steps, each with about
+        // twice as many busy lanes.  Owners queue (record index, owner lane) in shared memory; worker lane w takes item w, fetches the
         // owner's ray by shuffles and tests the record; hits meet in a 64-bit atomicMin per owner keyed by (t, item) --
         // among equal t the later item wins, as in the sequential order -- and the owner reads u, v back by shuffle.
         __shared__ uint32_t s_tri[TRACE_WARPS][32];
@@ -618,7 +617,6 @@ __global__ void __launch_bounds__(TRACE_THREADS, RTK_MIN_BLOCKS) trace_kernel(co
         int slot = incl - cnt;                                  // first queue slot of this lane's items
         const int total = min(__shfl_sync(FULL, incl, 31), 32);
         s_best[wi][lane] = ~0ull;
-        // (a predicated, unrolled version of this loop -- 3, 4 or 6 items per lane -- measured 1-5 % slower, r2_ab_runs.txt run 7)
         while (isT && tgy != 0 && slot < 32) {                  // highest bit first = the sequential test order
           const int tb = 31 - __clz((int)tgy);
           tgy &= ~(1u << tb);
@@ -769,14 +767,14 @@ static int launch_k(TraceParams p, cudaStream_t st) {
     int dev = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&g_num_sms, cudaDevAttrMultiProcessorCount, dev);
-    if (g_num_sms <= 0) g_num_sms = 148;
+    if (g_num_sms <= 0) g_num_sms = 132;
   }
-  p.tri_batch_min = p.curves ? g_tuning.curve_batch_min : g_tuning.tri_batch_min;
-  p.tri_wait_max = p.curves ? g_tuning.curve_wait_max : g_tuning.tri_wait_max;
+  p.tri_batch_min = p.curves == 2 ? g_tuning.curve_batch_min : p.curves ? g_tuning.point_batch_min : g_tuning.tri_batch_min;
+  p.tri_wait_max = p.curves == 2 ? g_tuning.curve_wait_max : p.curves ? g_tuning.point_wait_max : g_tuning.tri_wait_max;
   p.refill_min = g_tuning.refill_min;
   // persistent grid: a multiple of the SM count, capped by the work available
   const unsigned long long need = (p.n + TRACE_THREADS - 1) / TRACE_THREADS;
-  const unsigned long long cap = (unsigned long long)g_num_sms * g_tuning.blocks_per_sm;
+  const unsigned long long cap = (unsigned long long)g_num_sms * (p.curves == 2 ? g_tuning.curve_blocks_per_sm : g_tuning.blocks_per_sm);
   const unsigned blocks = (unsigned)(need < cap ? need : cap);
   // tiny launches (single-record API calls read a mapped pinned host record) skip the bulk prefetch
   p.use_prefetch = (p.n >= 1024 && g_tuning.use_tma) ? 1 : 0;

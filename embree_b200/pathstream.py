@@ -13,7 +13,7 @@ def load():
     global _lib
     if _lib is None:
         if not os.path.exists(LIB_PATH):
-            raise RuntimeError(f"{LIB_PATH} is missing: build it with `make -C embree_b200/csrc` (nvcc, sm_100a); there is no fallback")
+            raise RuntimeError(f"{LIB_PATH} is missing: build it with `make -C embree_b200/csrc` (nvcc, sm_90a); there is no fallback")
         d = C.CDLL(LIB_PATH)
         d.pts200_primary.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_ulonglong, C.c_uint, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p]
         d.pts200_bounce.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint, C.c_void_p, C.c_void_p]

@@ -1,4 +1,4 @@
-/* embree4_b200.h -- the C-ABI of the B200-native ray tracing kernel library.
+/* embree4_b200.h -- the C-ABI of the H100-native ray tracing kernel library.
  *
  * This is the drop-in boundary: a caller compiled against Embree 4.4.1's own
  * include/embree4/rtcore.h links against libembree4_b200.so unchanged for the
@@ -351,7 +351,7 @@ RTCB200_API void rtcb200Intersect1MDevice(RTCScene scene, struct RTCRayHit* d_ra
  * ray (primID = geomID = -1 on a miss) to compact_out[i] (32-byte aligned).  compact_out may be memory of ANOTHER GPU imported with
  * rtcb200PeerImport (the multi-GPU hit gather): the trace kernel stores the records itself, straight over NVLink when
  * the buffer is a peer's -- by default staged per 32-ray block in a local buffer and sent as 1 KB (eight full lines) when
- * the block is complete; rtcb200SetTuning("gather_mode", 0) selects one 256-bit store per record as its ray terminates.
+ * the block is complete; rtcb200SetTuning("gather_mode", 0) selects one 32-byte store per record as its ray terminates.
  * Either way, work enqueued on cuda_stream after this call sees the complete buffer. */
 RTCB200_API void rtcb200Intersect1MGatherDevice(RTCScene scene, struct RTCRayHit* d_rayhits, size_t M, struct RTCIntersectArguments* args, void* cuda_stream, void* compact_out);
 RTCB200_API void rtcb200Occluded1MDevice(RTCScene scene, struct RTCRay* d_rays, size_t M, struct RTCOccludedArguments* args, void* cuda_stream);
@@ -385,7 +385,8 @@ RTCB200_API void rtcb200ResetSceneStatCounters(RTCScene scene);
 /* number of kernel launches issued by this library since load (bench.py's gpu_launches) */
 RTCB200_API unsigned long long rtcb200GetLaunchCount(void);
 /* experiment knobs (process-wide): kernels "collapse_policy", "c_node", "c_tri", "sah_small", "tri_batch_min",
- * "tri_wait_max" ("curve_batch_min", "curve_wait_max": the same two for scenes with curves), "refill_min", "blocks_per_sm",
+ * "tri_wait_max" ("curve_batch_min", "curve_wait_max": the same two for scenes with curves, "point_batch_min",
+ * "point_wait_max" for scenes of points only), "refill_min", "blocks_per_sm" ("curve_blocks_per_sm" for scenes with curves),
  * "use_tma"; host-pointer pipeline "host_chunk_log2", "host_streams"; hit gather "gather_mode" (0 one store per record,
  * 1 complete 32-ray blocks as 1 KB stores); "tri_spread" (warp-wide triangle redistribution, on by default).
  * The defaults are the shipped, measured configuration.

@@ -6,10 +6,10 @@ anything produced here; only tests/, __graft_entry__.smoke() and bench.py's
 cpu_baseline / --impl reference legs may use it, as the checker / CPU baseline.
 
 This does NOT run the reference's own build system (CMake).  It compiles the
-reference sources *where they lie* under /root/reference with g++ through a
+reference sources *where they lie* under $EMBREE_REFERENCE with g++ through a
 ninja file that this script writes, following the source lists in
 kernels/CMakeLists.txt:33-195 and common/*/CMakeLists.txt, and the flags in
-common/cmake/gnu.cmake:12-92.  Nothing is copied out of /root/reference: the
+common/cmake/gnu.cmake:12-92.  Nothing is copied out of the reference tree: the
 three headers the reference's CMake would *generate* (rtcore_config.h,
 config.h, hash.h; templates kernels/rtcore_config.h.in, kernels/config.h.in,
 kernels/hash.h.in) are produced here by substituting the template variables
@@ -31,7 +31,7 @@ import re
 import subprocess
 import sys
 
-REF = os.environ.get("EMBREE_REFERENCE", "/root/reference")
+REF = os.environ.get("EMBREE_REFERENCE", "")
 HERE = os.path.dirname(os.path.abspath(__file__))
 
 MAIN_FILES = """
@@ -153,7 +153,7 @@ def main():
     ap.add_argument("-j", type=int, default=os.cpu_count())
     a = ap.parse_args()
     if not os.path.isdir(REF):
-        print(f"[build_ref] {REF} not present (GPU box?) -- using prebuilt oracle/_ref if any")
+        print(f"[build_ref] EMBREE_REFERENCE={REF!r} is not a directory -- using prebuilt oracle/_ref if any")
         return 0
     tag = "stat" if a.stat else "rel"
     out = os.path.join(HERE, "_ref")

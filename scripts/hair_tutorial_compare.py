@@ -1,5 +1,5 @@
 import subprocess, numpy as np, os, time
-ROOT='/root/repo'
+ROOT=os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 for t in (0,1,2):
     out=f'/tmp/hair_{t}.raw'
     t0=time.time()

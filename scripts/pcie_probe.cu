@@ -1,5 +1,5 @@
 // PCIe probe: linear vs strided (2D) copies of RTCRayHit streams, and zero-copy kernel gather/scatter.
-// Build: nvcc -O3 -gencode arch=compute_100a,code=sm_100a scripts/pcie_probe.cu -o scripts/_build/pcie_probe
+// Build: nvcc -O3 -gencode arch=compute_90a,code=sm_90a scripts/pcie_probe.cu -o scripts/_build/pcie_probe
 #include <cstdio>
 #include <cuda_runtime.h>
 #define CK(x) do { cudaError_t e = (x); if (e != cudaSuccess) { printf("%s: %s\n", #x, cudaGetErrorString(e)); return 1; } } while (0)
@@ -14,6 +14,8 @@ __global__ void scatter64(const uint4* __restrict__ src, uint4* __restrict__ dst
 }
 int main() {
   const size_t n = size_t(1) << 24;   // 16 Mi records, 1.6 GB
+  int sms = 0;
+  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, 0);
   char *h, *d;
   CK(cudaHostAlloc(&h, n * 96, cudaHostAllocMapped));
   CK(cudaMalloc(&d, n * 96));
@@ -31,17 +33,17 @@ int main() {
   time("D2H linear 96B", n * 96.0, [&] { cudaMemcpyAsync(h, d, n * 96, cudaMemcpyDeviceToHost, 0); });
   time("H2D 2D 48 of 96", n * 48.0, [&] { cudaMemcpy2DAsync(d, 96, h, 96, 48, n, cudaMemcpyHostToDevice, 0); });
   time("D2H 2D 64 of 96", n * 64.0, [&] { cudaMemcpy2DAsync(h + 32, 96, d + 32, 96, 64, n, cudaMemcpyDeviceToHost, 0); });
-  time("H2D kernel gather 48 of 96 (zero-copy)", n * 48.0, [&] { gather48<<<148 * 8, 256>>>((const uint4*)hd, (uint4*)d, n); });
-  time("D2H kernel scatter 64 of 96 (zero-copy)", n * 64.0, [&] { scatter64<<<148 * 8, 256>>>((const uint4*)d, (uint4*)hd, n); });
+  time("H2D kernel gather 48 of 96 (zero-copy)", n * 48.0, [&] { gather48<<<sms * 8, 256>>>((const uint4*)hd, (uint4*)d, n); });
+  time("D2H kernel scatter 64 of 96 (zero-copy)", n * 64.0, [&] { scatter64<<<sms * 8, 256>>>((const uint4*)d, (uint4*)hd, n); });
   time("duplex linear 96B both ways", n * 192.0, [&] {
     cudaMemcpyAsync(d, h, n * 48, cudaMemcpyHostToDevice, s1); cudaMemcpyAsync(h + n * 48, d + n * 48, n * 48, cudaMemcpyDeviceToHost, s2);
     cudaMemcpyAsync(d, h, n * 48, cudaMemcpyHostToDevice, s1); cudaMemcpyAsync(h + n * 48, d + n * 48, n * 48, cudaMemcpyDeviceToHost, s2);
     cudaStreamSynchronize(s1); cudaStreamSynchronize(s2); });
   time("duplex kernel gather48 || scatter64", n * 112.0, [&] {
-    gather48<<<148 * 4, 256, 0, s1>>>((const uint4*)hd, (uint4*)d, n / 2);
-    scatter64<<<148 * 4, 256, 0, s2>>>((const uint4*)(d + n * 48), (uint4*)(hd + n * 48), n / 2);
-    gather48<<<148 * 4, 256, 0, s1>>>((const uint4*)hd, (uint4*)d, n / 2);
-    scatter64<<<148 * 4, 256, 0, s2>>>((const uint4*)(d + n * 48), (uint4*)(hd + n * 48), n / 2);
+    gather48<<<sms * 4, 256, 0, s1>>>((const uint4*)hd, (uint4*)d, n / 2);
+    scatter64<<<sms * 4, 256, 0, s2>>>((const uint4*)(d + n * 48), (uint4*)(hd + n * 48), n / 2);
+    gather48<<<sms * 4, 256, 0, s1>>>((const uint4*)hd, (uint4*)d, n / 2);
+    scatter64<<<sms * 4, 256, 0, s2>>>((const uint4*)(d + n * 48), (uint4*)(hd + n * 48), n / 2);
     cudaStreamSynchronize(s1); cudaStreamSynchronize(s2); });
   return 0;
 }

@@ -5,7 +5,7 @@ GPU is idle?  Run under torchrun at 2, 4, 8 GPUs:
 
 Every rank copies a 2 GiB local buffer into its slice of a buffer that rank 0 allocated and exported through CUDA IPC
 (rtcb200PeerAlloc/Export/Import, the same plumbing the hit gather uses); the aggregate rate into rank 0 is printed for
-1 .. N-1 concurrent senders.  Compare with the ~175 GB/s the 8-GPU bench run implied (DESIGN.md section 7)."""
+1 .. N-1 concurrent senders, to compare with the rate at which rank 0 receives the hit gather of a multi-GPU bench run."""
 import ctypes as C
 import os
 import sys

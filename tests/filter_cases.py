@@ -1,8 +1,8 @@
 """Filter-callback scenarios shared by tests/golden/make_golden.py (run on the unmodified reference, outputs committed as
-tests/golden/filters.npz) and tests/test_filter.py (run on the B200 library through the same C-ABI and compared).
+tests/golden/filters.npz) and tests/test_filter.py (run on the CUDA library through the same C-ABI and compared).
 
 The callbacks are Python functions behind ctypes (rtc.FILTER_FUNCTION) that handle any N, as the reference's own test
-callback does (tutorials/verify/verify.cpp:2771-2786): the reference calls them with N = 1 or the packet width, the B200
+callback does (tutorials/verify/verify.cpp:2771-2786): the reference calls them with N = 1 or the packet width, the CUDA
 library always with N = 1.  The accept / reject rule is a pure function of the candidate's ids, so the final hit of a ray
 does not depend on the order in which a traversal meets the candidates."""
 import numpy as np

@@ -1,5 +1,5 @@
 """Generate golden input/output vectors by running the UNMODIFIED reference (oracle/_ref/libembree4.so.4, built
-from /root/reference by oracle/build_ref.py) in this container.  Committed outputs: tests/golden/*.npz.
+from the checkout EMBREE_REFERENCE names by oracle/build_ref.py).  Committed outputs: tests/golden/*.npz.
 
     python tests/golden/make_golden.py
 

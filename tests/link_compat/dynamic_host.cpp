@@ -1,5 +1,5 @@
 // Host driver for the reference's OWN tutorial device code tutorials/dynamic_scene/dynamic_scene_device.cpp (BASELINE configs[3]b), which
-// tests/link_compat/build.sh compiles untouched from /root/reference: an RTC_SCENE_FLAG_DYNAMIC | RTC_SCENE_FLAG_ROBUST scene (build quality
+// tests/link_compat/build.sh compiles untouched from $EMBREE_REFERENCE: an RTC_SCENE_FLAG_DYNAMIC | RTC_SCENE_FLAG_ROBUST scene (build quality
 // LOW) of a ground plane and 20 spheres with per-geometry build qualities, whose vertices the tutorial rewrites every frame through
 // rtcGetGeometryBufferData / rtcUpdateGeometryBuffer / rtcCommitGeometry before rtcCommitScene.  This file supplies what tutorial.cpp would
 // (g_device, g_stats, the camera of dynamic_scene.cpp:23-24) and renders a few frames of the animation to files, so the same tutorial code

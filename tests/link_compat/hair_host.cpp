@@ -1,5 +1,5 @@
 // Host driver for the reference's OWN tutorial device code tutorials/hair_geometry/hair_geometry_device.cpp (BASELINE configs[3]a),
-// which tests/link_compat/build.sh compiles untouched from /root/reference.  This file supplies what hair_geometry.cpp /
+// which tests/link_compat/build.sh compiles untouched from $EMBREE_REFERENCE.  This file supplies what hair_geometry.cpp /
 // tutorial.cpp / the scene loader would: g_device, g_stats, the lights and camera of models/furBall_A.ecs, and an ISPCScene
 // filled by hand with a procedural fur ball (the shipped model cannot travel to the GPU box) -- one hair set whose curve type is
 // chosen on the command line (round linear segments as in furBall_A.xml, flat or round cubic Bezier curves as the tutorials'

@@ -1,5 +1,5 @@
 // Host driver for the reference's OWN tutorial device code (tutorials/triangle_geometry/triangle_geometry_device.cpp =
-// BASELINE configs[0]), which tests/link_compat/build.sh compiles untouched from /root/reference: this file only supplies
+// BASELINE configs[0]), which tests/link_compat/build.sh compiles untouched from $EMBREE_REFERENCE: this file only supplies
 // what tutorials/common/tutorial/tutorial.cpp would (g_device, g_stats, the camera of triangle_geometry.cpp:23-24) and
 // writes the rendered frame to a file, so the same tutorial code can be linked once against the reference library
 // (golden image, generated in the container) and once against libembree4_b200.so (test on the GPU).

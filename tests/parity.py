@@ -144,6 +144,45 @@ def load_reference():
     return _ref
 
 
+REFERENCE_GOLDEN = os.path.join(ROOT, "tests", "golden", "reference")
+_WRITTEN = ("tfar", "Ng_x", "Ng_y", "Ng_z", "u", "v", "primID", "geomID", "instID")   # what a query writes into an RTCRayHit
+
+
+def reference_outputs(key, run, inputs=None, stride=1):
+    """The unmodified reference's answers to one test's seeded queries, so that the comparison with them runs with or without
+    the reference library.  run(R) performs the queries on the live reference and returns {name: array}.  Where oracle/_ref is
+    built, those live answers are returned for every query (and EMBREE_RECORD_GOLDEN=1 stores them); elsewhere the stored ones,
+    tests/golden/reference/<key>.npz: every `stride`-th row, of ray records only the fields a query writes, put back on top of
+    inputs[name] (the records the query started from).  Returns (answers, rows): the rows of the queries the answers belong to."""
+    path = os.path.join(REFERENCE_GOLDEN, key + ".npz")
+    R = load_reference()
+    if R is not None:
+        out = run(R)
+        if os.environ.get("EMBREE_RECORD_GOLDEN"):
+            flat = {}
+            for name, a in out.items():
+                if a.dtype.names:
+                    for f in (_WRITTEN if "primID" in a.dtype.names else ("tfar",)):
+                        flat[f"{name}.{f}"] = np.ascontiguousarray(a[f][::stride])
+                else:
+                    flat[name] = a
+            os.makedirs(REFERENCE_GOLDEN, exist_ok=True)
+            np.savez_compressed(path, **flat)
+        return out, slice(None)
+    rows = slice(None, None, stride)
+    z = np.load(path)
+    out = {}
+    for k in z.files:
+        name, _, f = k.partition(".")
+        if not f:
+            out[name] = z[k]
+            continue
+        if name not in out:
+            out[name] = inputs[name][rows].copy()
+        out[name][f] = z[k]
+    return out, rows
+
+
 def api_trace_mt(lib, scene, recs, nthreads, K=1, occluded=False, coherent=False, valid=None):
     """Loop lib's rtcIntersect1 / rtcOccluded1 / rtcIntersect{K} over `recs` on `nthreads` host threads (FTZ|DAZ set),
     i.e. how a host application drives the reference (BASELINE.md section 4)."""

@@ -1,7 +1,7 @@
 """Filter callbacks (SURVEY 8 a6 / a15 / a16): geometry filters, the arguments' filter, RTC_RAY_QUERY_FLAG_INVOKE_ARGUMENT_FILTER,
-rtcSetGeometryEnableFilterFunctionFromArguments -- through every host-pointer entry point of the B200 library, against
+rtcSetGeometryEnableFilterFunctionFromArguments -- through every host-pointer entry point of the CUDA library, against
 golden outputs of the unmodified reference (tests/golden/filters.npz, generator tests/golden/make_golden.py filters) and,
-when oracle/_ref travelled to the box, the reference run side by side with the same Python callbacks.
+when oracle/_ref is built, the reference run side by side with the same Python callbacks.
 Reference: kernels/geometry/filter.h:15-84, intersector_epilog.h:264-280,347-361; test model tutorials/verify/verify.cpp:2762-2838."""
 import ctypes as C
 import os
@@ -13,7 +13,7 @@ from embree_b200 import rtc, scenes
 from embree_b200.rtc import FILTER_FUNCTION, RayQueryContext, make_rayhits, rays_of
 from tests import filter_cases as fc
 from tests.conftest import ROOT, load_golden, load_golden_instances
-from tests.parity import compare_hits, load_reference
+from tests.parity import compare_hits, load_reference, reference_outputs
 
 pytestmark = pytest.mark.gpu
 MODES = ["1", "4", "8", "16", "1M", "4M", "8M", "16M"]
@@ -140,13 +140,14 @@ def test_filter_on_instanced_geometry(b200):
     got, rec = run(lib, dev)
     assert len(rec.calls) > 100
     assert all(c[1] == 0 and c[3] != 0xFFFFFFFF and c[4] == c[3] for c in rec.calls)   # child geomID 0, instID in hit == context
-    ref = load_reference()
-    if ref is None:
-        pytest.skip("oracle/_ref not present: the instanced filter case has no committed golden output")
-    rdev = ref.new_device(None)
-    want, rrec = run(ref, rdev)
-    ref.rtcReleaseDevice(rdev)
-    assert all(c[4] == c[3] for c in rrec.calls)
+
+    def run_reference(R):
+        rdev = R.new_device(None)
+        want, rrec = run(R, rdev)
+        R.rtcReleaseDevice(rdev)
+        assert all(c[4] == c[3] for c in rrec.calls)
+        return {"hits": want}
+    want = reference_outputs("filter_instanced", run_reference, {"hits": fc.number_rays(g["rays_in"].copy())})[0]["hits"]
     rep = compare_hits(want, got, 1e-4)
     assert rep["id_mismatch"] == 0 and rep["hit_miss_disagree"] == 0 and rep["tie"] <= 4, rep
 

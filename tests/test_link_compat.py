@@ -6,23 +6,43 @@ import subprocess
 import pytest
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-EXE = os.path.join(ROOT, "tests", "link_compat", "_bin", "embree_minimal")
+BIN = os.path.join(ROOT, "oracle", "_ref", "tutorials")   # tests/link_compat/build.sh output (needs EMBREE_REFERENCE at build time)
+EXE = os.path.join(BIN, "embree_minimal")
 LIB = os.path.join(ROOT, "embree_b200", "csrc", "libembree4_b200.so")
 
 
 def _ensure_built():
     subprocess.check_call([os.path.join(ROOT, "tests", "link_compat", "build.sh")])
     if not os.path.exists(EXE):
-        pytest.skip("reference sources not available and no prebuilt binary")
+        pytest.skip("tutorial binaries not built: build() needs EMBREE_REFERENCE to build them")
 
 
-def test_reference_tutorial_links_against_our_library():
-    _ensure_built()
-    needed = subprocess.check_output(["readelf", "-d", EXE]).decode()
+def _imports(exe):
+    und = subprocess.check_output(["nm", "-D", "--undefined-only", exe]).decode()
+    return sorted(l.split()[-1] for l in und.splitlines() if l.split()[-1].startswith("rtc"))
+
+
+def test_reference_tutorial_links_against_our_library(tmp_path):
+    """Where the reference checkout is available the tutorial itself is linked (tests/link_compat/build.sh); elsewhere a caller
+    importing exactly the rtc* symbols the tutorial imports (tests/golden/minimal_tutorial_imports.txt) is linked the same way,
+    with -lembree4 resolving to libembree4_b200.so."""
+    stored = [l.strip() for l in open(os.path.join(ROOT, "tests", "golden", "minimal_tutorial_imports.txt")) if l.strip() and not l.startswith("#")]
+    subprocess.check_call([os.path.join(ROOT, "tests", "link_compat", "build.sh")])
+    exe = EXE
+    if os.path.exists(EXE):
+        assert _imports(EXE) == stored
+    else:
+        src = tmp_path / "caller.c"
+        src.write_text("".join(f"extern void {n}(void);\n" for n in stored) +
+                       "void* volatile used[] = {" + ", ".join(f"(void*)&{n}" for n in stored) + "};\n"
+                       "int main(void) { return used[0] == 0; }\n")
+        os.symlink(LIB, tmp_path / "libembree4.so")
+        exe = str(tmp_path / "caller")
+        subprocess.check_call(["gcc", "-o", exe, str(src), f"-L{tmp_path}", "-lembree4", f"-Wl,-rpath,{os.path.dirname(LIB)}"])
+    needed = subprocess.check_output(["readelf", "-d", exe]).decode()
     assert "libembree4_b200.so" in needed and "libembree4.so.4" not in needed
-    und = subprocess.check_output(["nm", "-D", "--undefined-only", EXE]).decode()
-    wanted = sorted(l.split()[-1] for l in und.splitlines() if l.split()[-1].startswith("rtc"))
-    assert "rtcIntersect1" in wanted and "rtcCommitScene" in wanted
+    wanted = _imports(exe)
+    assert wanted == stored and "rtcIntersect1" in wanted and "rtcCommitScene" in wanted
     exported = subprocess.check_output(["nm", "-D", "--defined-only", LIB]).decode()
     have = set(l.split()[-1] for l in exported.splitlines())
     assert not [w for w in wanted if w not in have]
@@ -37,7 +57,7 @@ def test_reference_tutorial_runs_on_the_gpu():
     assert "Did not find any intersection." in out, out
 
 
-TUT = os.path.join(ROOT, "tests", "link_compat", "_bin", "embree_triangle_geometry")
+TUT = os.path.join(BIN, "embree_triangle_geometry")
 GOLDEN_FRAME = os.path.join(ROOT, "tests", "golden", "triangle_geometry_160x120.raw")
 
 
@@ -68,7 +88,7 @@ def test_triangle_geometry_tutorial_renders_the_reference_frame(tmp_path):
     assert diff.sum() <= 0.003 * w.size and not (diff & ~edge).any(), f"{diff.sum()} pixels differ, {(diff & ~edge).sum()} of them off an edge"
 
 
-POINTS = os.path.join(ROOT, "tests", "link_compat", "_bin", "embree_point_geometry")
+POINTS = os.path.join(BIN, "embree_point_geometry")
 
 
 @pytest.mark.gpu
@@ -99,7 +119,7 @@ def test_point_geometry_tutorial_renders_the_reference_frame(tmp_path):
     assert big.sum() <= 0.005 * w.size and diff.sum() <= 0.03 * w.size and not (big & ~edge).any(), f"{diff.sum()} pixels differ, {big.sum()} by more than one step, {(big & ~edge).sum()} of them off an edge"
 
 
-HAIR = os.path.join(ROOT, "tests", "link_compat", "_bin", "embree_hair_geometry")
+HAIR = os.path.join(BIN, "embree_hair_geometry")
 
 
 @pytest.mark.gpu
@@ -137,7 +157,7 @@ def test_hair_geometry_tutorial_renders_the_reference_frame(tmp_path, ctype, nam
         assert same >= 0.93 and mean_diff < 1.0, (name, same, mean_diff)
 
 
-DYN = os.path.join(ROOT, "tests", "link_compat", "_bin", "embree_dynamic_scene")
+DYN = os.path.join(BIN, "embree_dynamic_scene")
 
 
 @pytest.mark.gpu

@@ -35,7 +35,7 @@ def test_pathstream_library_exports():
     for name in ("pts200_primary", "pts200_bounce", "pts200_shade"):
         assert hasattr(lib, name)
     out = subprocess.run(["cuobjdump", "-lelf", pathstream.LIB_PATH], stdout=subprocess.PIPE, text=True).stdout
-    assert "sm_100a" in out and all("sm_100a" in l for l in out.splitlines() if "sm_" in l), out
+    assert "sm_90a" in out and all("sm_90a" in l for l in out.splitlines() if "sm_" in l), out
 
 
 @pytest.mark.gpu

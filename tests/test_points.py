@@ -151,9 +151,8 @@ def test_point_api_errors_and_updates(b200):
 def test_instanced_curves_and_points(b200, oracle):
     """Instances of a scene holding every curve and point kind (round / flat linear, flat / round Bezier, sphere / disc / oriented disc
     points) under rotation, non-uniform scale and translation, with instance and geometry masks: hits (ids, instID, t, u, v, Ng in
-    object space) equal the C oracle's -- which tests/test_oracle.py pins to the live reference on the same scene -- and, when
-    oracle/_ref travelled to the box, the live reference's too."""
-    from tests.parity import build_instanced_hair, instanced_hair_scene, load_reference
+    object space) equal the C oracle's and the reference's (live when oracle/_ref is built, else its stored answers)."""
+    from tests.parity import build_instanced_hair, instanced_hair_scene, reference_outputs
     lib, dev = b200
     S = instanced_hair_scene()
     top, child, keep = build_instanced_hair(lib, dev, S)
@@ -165,15 +164,17 @@ def test_instanced_curves_and_points(b200, oracle):
     lib.rtcGetSceneBounds(top, C.byref(b))
     got_b = np.array([b.lower_x, b.lower_y, b.lower_z, b.upper_x, b.upper_y, b.upper_z], np.float32)
     assert np.allclose(got_b, ot.bounds(), rtol=1e-5, atol=1e-5)
-    refs = [("oracle", want, wocc)]
-    R = load_reference()
-    if R is not None:
+
+    def run(R):
         rdev = R.new_device(None)
         rtop, rchild, rkeep = build_instanced_hair(R, rdev, S)
-        refs.append(("reference", R.intersect(rtop, S["rays"].copy(), "1"), R.occluded(rtop, rays_of(S["rays"]), "1")))
+        out = {"hits": R.intersect(rtop, S["rays"].copy(), "1"), "occ": R.occluded(rtop, rays_of(S["rays"]), "1")}
         R.rtcReleaseScene(rtop)
         R.rtcReleaseScene(rchild)
         R.rtcReleaseDevice(rdev)
+        return out
+    ref = reference_outputs("instanced_curves_and_points", run, {"hits": S["rays"], "occ": rays_of(S["rays"])})[0]
+    refs = [("oracle", want, wocc), ("reference", ref["hits"], ref["occ"])]
     for mode in ("1M", "8", "16M"):
         got = lib.intersect(top, S["rays"].copy(), mode)
         occ = lib.occluded(top, rays_of(S["rays"]), mode)

@@ -13,7 +13,7 @@ pytestmark = pytest.mark.gpu
 def test_gather_records(b200):
     """rtcb200Intersect1MGatherDevice: the compact 32-byte record per ray {tfar, Ng, u, v, primID, geomID} equals the
     RTCRayHit result in both delivery modes ("gather_mode" 1: blocks staged in shared memory and stored as 1 KB, the
-    default; 0: one 256-bit store per record), with work enqueued on the caller's stream after the call seeing the complete
+    default; 0: one 32-byte store per record), with work enqueued on the caller's stream after the call seeing the complete
     buffer; a ray count that is not a multiple of 32 exercises the partial tail block."""
     import torch
     from embree_b200 import sharding
