@@ -11,6 +11,22 @@
 
 namespace rtk {
 
+// what the leaf records of a GeomDesc are and which test they take (build.cu primref_gen / leaf_pack, trace.cu curve_record_test)
+enum PrimKind : uint32_t {
+  PRIM_TRIANGLE = 0,        // triangle or quad mesh (a quad is stored as two triangle records)
+  PRIM_ROUND_LINEAR = 1,    // cone-sphere segment
+  PRIM_FLAT_LINEAR = 2,     // ray-facing ribbon segment
+  PRIM_FLAT_CUBIC = 3,      // tessellated ribbon, one record per segment
+  PRIM_ROUND_CUBIC = 4,     // sweep, one record per first-level sub-segment
+  PRIM_SPHERE = 5,          // point kinds: point_test's point type is kind - PRIM_SPHERE
+  PRIM_DISC = 6,            // ray-facing disc
+  PRIM_ORIENTED_DISC = 7,   // disc with a normal (in `tangents`, stride `tstride`)
+};
+// The kernels write `kind >= PRIM_SPHERE` out instead of calling point_record: even inlined, the call changes how the compiler lays
+// out their if-chains over the kinds.
+RT_HD constexpr bool curve_record(uint32_t kind) { return kind >= PRIM_ROUND_LINEAR && kind <= PRIM_ROUND_CUBIC; }
+RT_HD constexpr bool point_record(uint32_t kind) { return kind >= PRIM_SPHERE; }   // PRIM_ORIENTED_DISC is the last kind
+
 // one enabled triangle mesh, buffers already resident on the device (raw bytes, caller's stride honoured:
 // kernels/common/buffer.h BufferView semantics)
 struct GeomDesc {
@@ -29,8 +45,7 @@ struct GeomDesc {
   // round linear curves (RTC_GEOMETRY_TYPE_ROUND_LINEAR_CURVE): verts = float4 (xyz, radius), idx = first vertex of each
   // segment, ntris = segments; `flags` = one neighbour-flag byte per segment (device).  The vertex buffer stays resident
   // after the build: the trace kernel fetches the neighbour vertices from it.
-  uint32_t is_curve = 0;   // 1 round linear (cone-sphere), 2 flat linear (ray-facing ribbon), 3 flat cubic (tessellated ribbon), 4 round cubic (sweep),
-                           // 5 sphere point, 6 ray-facing disc point, 7 oriented disc point (normals in `tangents`, stride `tstride`)
+  uint32_t kind = PRIM_TRIANGLE;   // PrimKind of the records
   const uint8_t* flags = nullptr;
   // flat cubic curves (RTC_GEOMETRY_TYPE_FLAT_BEZIER / _BSPLINE / _CATMULL_ROM / _HERMITE_CURVE): idx = first of the four
   // control vertices (Hermite: of the two vertex / tangent pairs), `basis` = rt_core.cuh CurveBasis of the control points,

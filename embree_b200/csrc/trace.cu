@@ -120,18 +120,18 @@ __device__ __noinline__ bool round_record_test(const GeomDesc& d, const Ray& r, 
   return round_cubic_test(r.ox, r.oy, r.oz, r.dx, r.dy, r.dz, r.tnear, tfar, cp, d.basis, h, lane);
 }
 __device__ __noinline__ bool curve_record_test(const GeomDesc& d, const Ray& r, float tfar, const uint4& a, const uint4& b, const uint4& c, CurveHit& h) {
-  if (d.is_curve >= 5)   // point primitives (sphere / ray-facing disc / oriented disc): the record holds everything (build.cu leaf_pack)
+  if (d.kind >= PRIM_SPHERE)   // point primitives (sphere / ray-facing disc / oriented disc): the record holds everything (build.cu leaf_pack)
     return point_test(r.ox, r.oy, r.oz, r.dx, r.dy, r.dz, r.tnear, tfar, __uint_as_float(a.x), __uint_as_float(a.y), __uint_as_float(a.z),
-                      __uint_as_float(c.x), __uint_as_float(b.x), __uint_as_float(b.y), __uint_as_float(b.z), (int)d.is_curve - 5, h);
-  if (d.is_curve == 4) return round_record_test(d, r, tfar, c.z, (int)c.x, h);   // c.x: this record's first-level sub-segment
-  if (d.is_curve == 3) {   // flat cubic curve (Bezier / B-spline / Catmull-Rom / Hermite): control points from the resident vertex buffer
+                      __uint_as_float(c.x), __uint_as_float(b.x), __uint_as_float(b.y), __uint_as_float(b.z), (int)(d.kind - PRIM_SPHERE), h);
+  if (d.kind == PRIM_ROUND_CUBIC) return round_record_test(d, r, tfar, c.z, (int)c.x, h);   // c.x: this record's first-level sub-segment
+  if (d.kind == PRIM_FLAT_CUBIC) {   // flat cubic curve (Bezier / B-spline / Catmull-Rom / Hermite): control points from the resident vertex buffer
     CurveVtx cp[4];
     load_cubic_cp(d, c.z, cp);
     return flat_cubic_test(r.ox, r.oy, r.oz, r.dx, r.dy, r.dz, r.tnear, tfar, cp, d.basis, (int)d.tess, d.basis_tab, h, (int)c.x);   // c.x: this record's segment
   }
   const CurveVtx v0{__uint_as_float(a.x), __uint_as_float(a.y), __uint_as_float(a.z), __uint_as_float(c.x)};
   const CurveVtx v1{__uint_as_float(b.x), __uint_as_float(b.y), __uint_as_float(b.z), __uint_as_float(c.y)};
-  if (d.is_curve == 2)   // RTC_GEOMETRY_TYPE_FLAT_LINEAR_CURVE: ray-facing ribbon, no neighbours involved
+  if (d.kind == PRIM_FLAT_LINEAR)   // RTC_GEOMETRY_TYPE_FLAT_LINEAR_CURVE: ray-facing ribbon, no neighbours involved
     return flat_curve_test(r.ox, r.oy, r.oz, r.dx, r.dy, r.dz, r.tnear, tfar, v0, v1, h);
   const uint32_t vid = c.z & 0x3FFFFFFFu;
   const bool hasL = (c.z >> 30) & 1u, hasR = (c.z >> 31) & 1u;
@@ -344,21 +344,21 @@ __global__ void __launch_bounds__(TRACE_THREADS, RTK_MIN_BLOCKS) trace_kernel(co
         hit.primID = a.w; hit.geomID = b.w;
         uint32_t instID = p.instID, instPrimID = p.instPrimID;
         float lox = r.ox, loy = r.oy, loz = r.oz;   // ray origin in the space the record's triangle lives in
-        bool is_curve = false;
+        bool curve_hit = false;
         if (GENERAL) {   // ids through the descriptor; Ng stays in OBJECT space as in the reference
           const GeomDesc& d = p.descs[b.w];
           hit.geomID = d.geomID;
-          if (GENERAL == 2 && d.is_curve) {   // the normal of a curve hit depends on which surface was hit: kept from the winning test
+          if (GENERAL == 2 && d.kind != PRIM_TRIANGLE) {   // the normal of a curve hit depends on which surface was hit: kept from the winning test
             hit.ngx = __uint_as_float(s_lane[GENERAL == 2 ? 9 : 0][threadIdx.x]); hit.ngy = __uint_as_float(s_lane[GENERAL == 2 ? 10 : 0][threadIdx.x]);
             hit.ngz = __uint_as_float(s_lane[GENERAL == 2 ? 11 : 0][threadIdx.x]);
-            is_curve = true;
+            curve_hit = true;
           }
           if (d.has_xfm) {
             instID = d.instID; instPrimID = 0u;   // instance_id_stack::push(context, instID, 0)
             if (ROBUST) { Ray lr = full_ray(); to_object_space(d, lr); lox = lr.ox; loy = lr.oy; loz = lr.oz; }
           }
         }
-        if (is_curve) {
+        if (curve_hit) {
         } else if (ROBUST) {   // stable_triangle_normal of the origin-relative edges, exactly as in tri_test_pluecker
           const float v0x = sub_rn(__uint_as_float(a.x), lox), v0y = sub_rn(__uint_as_float(a.y), loy), v0z = sub_rn(__uint_as_float(a.z), loz);
           const float v1x = sub_rn(__uint_as_float(b.x), lox), v1y = sub_rn(__uint_as_float(b.y), loy), v1z = sub_rn(__uint_as_float(b.z), loz);
@@ -372,7 +372,7 @@ __global__ void __launch_bounds__(TRACE_THREADS, RTK_MIN_BLOCKS) trace_kernel(co
           hit.ngy = msub(e2z, e1x, mul_rn(e2x, e1z));
           hit.ngz = msub(e2x, e1y, mul_rn(e2y, e1x));
         }
-        if (GENERAL && !is_curve && (a.w >> 31)) {   // quad halves share the quad's primID; the second one has flipped winding
+        if (GENERAL && !curve_hit && (a.w >> 31)) {   // quad halves share the quad's primID; the second one has flipped winding
           hit.primID = a.w & 0x7FFFFFFFu;
           hit.ngx = -hit.ngx; hit.ngy = -hit.ngy; hit.ngz = -hit.ngz;
         }
@@ -407,7 +407,7 @@ __global__ void __launch_bounds__(TRACE_THREADS, RTK_MIN_BLOCKS) trace_kernel(co
     bool visible = (c.w & lr.mask) != 0;             // ray mask (intersector_epilog.h:256-262)
     if (GENERAL) {   // b.w = descriptor index: instance mask (instance_intersector.cpp:19-22) + object-space ray
       const GeomDesc& d = p.descs[b.w];
-      if (GENERAL == 2 && d.is_curve) {   // RTC_GEOMETRY_TYPE_ROUND_LINEAR_CURVE: cone-sphere test, u along the segment, v = 0
+      if (GENERAL == 2 && d.kind != PRIM_TRIANGLE) {   // RTC_GEOMETRY_TYPE_ROUND_LINEAR_CURVE: cone-sphere test, u along the segment, v = 0
         CurveHit ch;
         visible = visible && (d.inst_mask & lr.mask) != 0;   // an instanced curve / point geometry: the instance's mask as well,
         if (d.has_xfm) to_object_space(d, lr);               // and the test runs on the object-space ray (t is unchanged)
