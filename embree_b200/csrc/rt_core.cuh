@@ -81,6 +81,7 @@ struct Hit {  // what a closest-hit query commits (intersector_epilog.h:285-299)
 };
 
 constexpr float kMinRcpInput = 1e-18f;   // common/math/constants.h:18
+constexpr float kRcpOfMin = 5e17f;         // |1/dir| at or above this: the direction component is (nearly) the rcp_safe clamp
 constexpr float kFltLarge = 1.844E18f;   // common/math/constants.h:21
 constexpr uint32_t kInvalidID = 0xFFFFFFFFu;
 constexpr int kMaxLeafTris = 3;
@@ -141,6 +142,38 @@ RT_HD float sub_rn(float a, float b) {
 #endif
 }
 RT_HD float msub(float a, float b, float c) { return fma_rn(a, b, -c); }            // a*b - c
+// a - b and a * b rounded towards -inf (_rd) or +inf (_ru).  The host versions round to nearest and step one float
+// towards the required side when the exact error of that rounding (TwoSum / FMA, both exact) has the wrong sign.
+RT_HD float sub_rd(float a, float b) {
+#if defined(__CUDA_ARCH__)
+  return __fsub_rd(a, b);
+#else
+  volatile float r = a - b; volatile float bb = r - a; const float e = (a - (r - bb)) + (-b - bb);
+  return e < 0.0f ? nextafterf(r, -INFINITY) : r;
+#endif
+}
+RT_HD float sub_ru(float a, float b) {
+#if defined(__CUDA_ARCH__)
+  return __fsub_ru(a, b);
+#else
+  volatile float r = a - b; volatile float bb = r - a; const float e = (a - (r - bb)) + (-b - bb);
+  return e > 0.0f ? nextafterf(r, INFINITY) : r;
+#endif
+}
+RT_HD float mul_rd(float a, float b) {
+#if defined(__CUDA_ARCH__)
+  return __fmul_rd(a, b);
+#else
+  volatile float r = a * b; return fmaf(a, b, -r) < 0.0f ? nextafterf(r, -INFINITY) : r;
+#endif
+}
+RT_HD float mul_ru(float a, float b) {
+#if defined(__CUDA_ARCH__)
+  return __fmul_ru(a, b);
+#else
+  volatile float r = a * b; return fmaf(a, b, -r) > 0.0f ? nextafterf(r, INFINITY) : r;
+#endif
+}
 RT_HD float dot3(float ax, float ay, float az, float bx, float by, float bz) {      // vec3.h:204
   return fma_rn(ax, bx, fma_rn(ay, by, mul_rn(az, bz)));
 }
@@ -1267,12 +1300,37 @@ RT_HD uint32_t node_hitmask(const uint32_t* w, float ox, float oy, float oz, flo
                             bool negy, bool negz, float tnear, float tfar, uint32_t oct_inv) {
   const uint32_t e = w[3];
   // per-axis: t = q * (2^e * idir) + (p - org) * idir
+  //
+  // Conservative to exact arithmetic (u = 2^-24).  Rounded to nearest, (p - org) * idir carries an absolute error of
+  // up to ~2u |(p - org) idir|: with the origin inside a large node, far from p and close to a child face, that exceeds
+  // any relative pad on the plane distance, and a box the ray enters is culled.  So the offset is computed twice, with
+  // directed rounding: bn <= (p - org) idir <= bf exactly (the subtraction and the product are both rounded away from
+  // the side each bound must lie on; which rounding of p - org gives which bound depends on the sign of idir).  Near
+  // planes use bn, far planes bf.  What remains is relative: idir = (1/d)(1 + d0) and the FMA's rounding (1 + d1),
+  // |di| <= u, so every computed near distance is <= max(t*, 0) (1 + u)^2 and every far distance >= t* (1 - u)^2
+  // for t* >= 0 (t* the exact distance to the plane p + q 2^e).  The factor 1 + 6u on tmax covers both ends and its own
+  // rounding: (1 - u)^3 (1 + 6u) >= (1 + u)^2, so tmin <= tmax whenever the exact interval is non-empty.
+  // The triangle, quad, curve and point tests round too: they accept hits up to about an ulp of the coordinates outside
+  // a primitive's box, which is an absolute error of the same kind.  So on every axis whose direction is not rcp_safe's
+  // clamp the offsets are widened by 2^-22 of their magnitude (bn - 4u|bn|, bf + 4u|bf|); with that margin no hit the
+  // reference finds is lost in the grid-aligned scenes of tests/test_traversal_bounds.py.  On a clamped axis (|1/dir| >= kRcpOfMin) the offsets stay exact: a ray lying in a face plane with a
+  // zero direction component leaves or enters the box as the clamped direction says, and where p - org and the product
+  // are exact the test equals the unpadded one.  The per-child work is unchanged.
   const float sx = u2f((e & 0xFFu) << 23) * idx;
   const float sy = u2f(((e >> 8) & 0xFFu) << 23) * idy;
   const float sz = u2f(((e >> 16) & 0xFFu) << 23) * idz;
-  const float bx = (u2f(w[0]) - ox) * idx;
-  const float by = (u2f(w[1]) - oy) * idy;
-  const float bz = (u2f(w[2]) - oz) * idz;
+  const float px = u2f(w[0]), py = u2f(w[1]), pz = u2f(w[2]);
+  const float dlx = sub_rd(px, ox), dhx = sub_ru(px, ox);
+  const float dly = sub_rd(py, oy), dhy = sub_ru(py, oy);
+  const float dlz = sub_rd(pz, oz), dhz = sub_ru(pz, oz);
+  const float kx = fabsf(idx) < kRcpOfMin ? 0x1p-22f : 0.0f, ky = fabsf(idy) < kRcpOfMin ? 0x1p-22f : 0.0f,
+              kz = fabsf(idz) < kRcpOfMin ? 0x1p-22f : 0.0f;
+  const float dnx = mul_rd(negx ? dhx : dlx, idx), dfx = mul_ru(negx ? dlx : dhx, idx);   // bounds of (p - org) idir
+  const float dny = mul_rd(negy ? dhy : dly, idy), dfy = mul_ru(negy ? dly : dhy, idy);
+  const float dnz = mul_rd(negz ? dhz : dlz, idz), dfz = mul_ru(negz ? dlz : dhz, idz);
+  const float bnx = fma_rn(-kx, fabsf(dnx), dnx), bfx = fma_rn(kx, fabsf(dfx), dfx);       // near / far plane offsets
+  const float bny = fma_rn(-ky, fabsf(dny), dny), bfy = fma_rn(ky, fabsf(dfy), dfy);
+  const float bnz = fma_rn(-kz, fabsf(dnz), dnz), bfz = fma_rn(kz, fabsf(dfz), dfz);
   uint32_t leaf = 0, slots = 0;
 #pragma unroll
   for (int half = 0; half < 2; ++half) {
@@ -1285,15 +1343,14 @@ RT_HD uint32_t node_hitmask(const uint32_t* w, float ox, float oy, float oz, flo
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
       const int sh = 8 * j;
-      const float tnx = fma_rn((float)((nx >> sh) & 0xFFu), sx, bx);
-      const float tny = fma_rn((float)((ny >> sh) & 0xFFu), sy, by);
-      const float tnz = fma_rn((float)((nz >> sh) & 0xFFu), sz, bz);
-      const float tfx = fma_rn((float)((fx >> sh) & 0xFFu), sx, bx);
-      const float tfy = fma_rn((float)((fy >> sh) & 0xFFu), sy, by);
-      const float tfz = fma_rn((float)((fz >> sh) & 0xFFu), sz, bz);
+      const float tnx = fma_rn((float)((nx >> sh) & 0xFFu), sx, bnx);
+      const float tny = fma_rn((float)((ny >> sh) & 0xFFu), sy, bny);
+      const float tnz = fma_rn((float)((nz >> sh) & 0xFFu), sz, bnz);
+      const float tfx = fma_rn((float)((fx >> sh) & 0xFFu), sx, bfx);
+      const float tfy = fma_rn((float)((fy >> sh) & 0xFFu), sy, bfy);
+      const float tfz = fma_rn((float)((fz >> sh) & 0xFFu), sz, bfz);
       const float tmin = fmaxf(fmaxf(tnx, tny), fmaxf(tnz, tnear));
-      // pad the exit distance by 2 ulp so rounding in the FMAs can never cull a box that exact arithmetic
-      // accepts (the reference's robust mode pads by 3 ulp, node_intersector1.h:106-110)
+      // 1.0000003f = 1 + 6u: the relative part of the bound above, for both ends of the interval
       const float tmax = fminf(fminf(tfx, tfy), fminf(tfz, tfar)) * 1.0000003f;
       if (tmin <= tmax) {
         leaf |= node_leafmask_raw(w, 4 * half + j);

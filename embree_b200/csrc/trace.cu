@@ -89,7 +89,7 @@ struct RayIO {
 };
 
 // rcp_safe with the reference's own recipe: hardware approximation + one Newton step (common/simd/vfloat4_sse2.h:304-323)
-// instead of an IEEE division; the slab test is padded by 2 ulp, so the ~1 ulp error of 1/dir cannot cull a box wrongly.
+// instead of an IEEE division: __frcp_rn is correctly rounded, the 1/dir error that node_hitmask's pads are derived for.
 __device__ __forceinline__ float rcp_safe_fast(float d) {
   const float x = fabsf(d) < kMinRcpInput ? kMinRcpInput : d;
   const float r = __frcp_rn(x);

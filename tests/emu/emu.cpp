@@ -1,7 +1,7 @@
 // emu.cpp -- TEST TOOL ONLY: runs the host instantiation of embree_b200/csrc/rt_core.cuh serially on the CPU so the
 // shared core routines (LBVH node construction, BVH8 collapse + slot assignment + box quantisation, the traversal
 // loop and the triangle test) can be debugged in a container without a GPU.  It is compiled by tests/emu/build.sh
-// into tests/emu/_build/libemu.so, loaded only by tests/test_emu_*.py, never by the product and never by bench.py.
+// into tests/emu/_build/libemu.so, loaded only by the tests (the `emu` fixture), never by the product and never by bench.py.
 // The GPU-only parts (radix sort, atomics-based refit, level scheduling) are replaced by trivial serial code here.
 #include <math.h>
 #include <stdint.h>
@@ -213,6 +213,39 @@ void emu_trace(void* h, void* rays, uint64_t n, int occluded, uint64_t* stats) {
     memcpy(rec + 48, h4, 20);
     uint32_t ids[4] = {hit.primID, hit.geomID, 0xFFFFFFFFu, 0xFFFFFFFFu};
     memcpy(rec + 68, ids, 16);
+  }
+}
+
+// One BVH8 node over n <= 8 child boxes (float[n][6]: lo xyz, hi xyz), built as collapse_node builds it: the node box is
+// the union of the children, assign_slots orders them, encode_node_boxes quantises them.  Each ray (float[8]: org xyz,
+// tnear, dir xyz, tfar) is set up as traverse() sets it up and tested with node_hitmask; out[i] bit c = child c passed.
+void emu_node_hitmask(const float* boxes, int n, const float* rays, uint64_t m, uint32_t* out) {
+  ChildBox cb[8];
+  float plo[3] = {INFINITY, INFINITY, INFINITY}, phi[3] = {-INFINITY, -INFINITY, -INFINITY};
+  for (int c = 0; c < n; ++c)
+    for (int a = 0; a < 3; ++a) {
+      cb[c].lo[a] = boxes[6 * c + a]; cb[c].hi[a] = boxes[6 * c + 3 + a];
+      plo[a] = fminf(plo[a], cb[c].lo[a]); phi[a] = fmaxf(phi[a], cb[c].hi[a]);
+    }
+  uint8_t slot_of[8];
+  assign_slots(cb, n, plo, phi, slot_of);
+  Node8 nd;
+  for (int k = 0; k < 24; ++k) nd.w[k] = 0;
+  encode_node_boxes(nd, plo, phi, cb, slot_of, n);
+  uint32_t imask = 0;
+  for (int c = 0; c < n; ++c) imask |= 1u << slot_of[c];
+  nd.w[3] = (nd.w[3] & 0x00FFFFFFu) | (imask << 24);   // every child internal: the hit slots come back in bits 31:24
+  for (uint64_t i = 0; i < m; ++i) {
+    const float* r = rays + 8 * i;
+    const float idx = rcp_safe(r[4]), idy = rcp_safe(r[5]), idz = rcp_safe(r[6]);
+    const bool negx = idx < 0.0f, negy = idy < 0.0f, negz = idz < 0.0f;
+    const uint32_t oct = (negx ? 1u : 0u) | (negy ? 2u : 0u) | (negz ? 4u : 0u);
+    const uint32_t hm = node_hitmask(nd.w, r[0], r[1], r[2], idx, idy, idz, negx, negy, negz, fmaxf(r[3], 0.0f),
+                                     fmaxf(r[7], 0.0f), 7u - oct);
+    const uint32_t slots = xor_permute8(hm >> 24, 7u - oct);
+    uint32_t mask = 0;
+    for (int c = 0; c < n; ++c) mask |= ((slots >> slot_of[c]) & 1u) << c;
+    out[i] = mask;
   }
 }
 

@@ -255,7 +255,7 @@ def explain_hit_miss(oracle, rays, want, got, single_prim_scene):
       * got hits, want misses: `single_prim_scene(geomID, primID, instID)` builds an oracle scene that holds ONLY the
         primitive the GPU reports; the reference's own triangle arithmetic must accept it there with bit-equal t, u, v.
         Then the full-scene miss is the reference's non-conservative fast box test culling that leaf by a rounding error
-        (node_intersector1.h:484-531 carries no padding; ours is padded by 2 ulp), not a wrong GPU hit.
+        (node_intersector1.h:484-531 carries no padding; ours is padded by a bound on its rounding error), not a wrong GPU hit.
     Returns (lost, unexplained_extra)."""
     wh = want["geomID"] != 0xFFFFFFFF
     gh = got["geomID"] != 0xFFFFFFFF
