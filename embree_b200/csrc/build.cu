@@ -317,13 +317,19 @@ __global__ void __launch_bounds__(256) primref_gen(const GeomDesc* __restrict__ 
     pr.hix = hi[0]; pr.hiy = hi[1]; pr.hiz = hi[2]; pr.valid = ok ? 1u : 0u;
     out[p] = pr;
   }
+  // an invalid primitive has no box: the curve branches above compute one and only then reject it when it crosses +-kFltLarge
+  // (isvalid(b), scene_curves.h:527), and that box must not reach the scene bounds (the SAH root's box) or the API bounds
+  if (!ok) {
+#pragma unroll
+    for (int a = 0; a < 3; ++a) { lo[a] = INFINITY; hi[a] = -INFINITY; }
+  }
   // warp reduce, then one set of atomics per warp
   float c_lo[3], c_hi[3];
 #pragma unroll
   for (int a = 0; a < 3; ++a) { c_lo[a] = ok ? lo[a] + hi[a] : INFINITY; c_hi[a] = ok ? lo[a] + hi[a] : -INFINITY; }
   float a_lo[3], a_hi[3];   // API-visible bounds: instanced triangles are represented by their instance box (host side)
 #pragma unroll
-  for (int a = 0; a < 3; ++a) { a_lo[a] = skipb ? INFINITY : (own_api ? alo[a] : lo[a]); a_hi[a] = skipb ? -INFINITY : (own_api ? ahi[a] : hi[a]); }
+  for (int a = 0; a < 3; ++a) { a_lo[a] = (skipb || !ok) ? INFINITY : (own_api ? alo[a] : lo[a]); a_hi[a] = (skipb || !ok) ? -INFINITY : (own_api ? ahi[a] : hi[a]); }
   unsigned cnt = ok ? 1u : 0u;
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) {
@@ -883,7 +889,7 @@ int build_scene(SceneGPU& s, const GeomDesc* geoms, int ngeoms, BuilderKind kind
   float ms = 0;
   cudaEventElapsedTime(&ms, ev0, ev1);
   s.nodes = d_final.p; s.tris = d_tris.p; d_final.p = nullptr; d_tris.p = nullptr;   // ownership moves to the scene
-  if (s.general) { s.d_descs = d_geoms.p; d_geoms.p = nullptr; }
+  if (s.general) { s.d_descs = d_geoms.p; d_geoms.p = nullptr; s.num_descs = (uint32_t)ngeoms; }
   s.num_nodes = end; s.num_tris = n; s.root_valid = 1;
   s.build_ms = ms; s.sah_cost = hinfo.sah; s.max_depth = depth;
   // kept for refit_scene(): which primitive every triangle record came from, and the level ranges of the node array

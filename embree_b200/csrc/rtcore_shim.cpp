@@ -1539,6 +1539,47 @@ void rtcb200GetSceneStats(RTCScene sc, struct RTCB200SceneStats* o) {
   }
   SCENE_END
 }
+static void scene_layout(const rtk::SceneGPU& g, RTCB200SceneLayout* o) {
+  memset(o, 0, sizeof *o);
+  if (g.root_valid) {
+    o->num_nodes = g.num_nodes; o->num_records = g.num_tris;
+    o->num_descs = g.d_descs ? g.num_descs : 0u;
+    o->num_levels = (unsigned)g.levels.size();
+    o->num_subs = g.builder == 3 ? (unsigned)g.sub_node_off.size() : 0u;
+    o->top_nodes = g.builder == 3 ? g.top_cap : 0u;
+  }
+  o->max_depth = g.max_depth; o->general = (unsigned)g.general; o->robust = (unsigned)g.robust; o->builder = g.builder;
+}
+void rtcb200GetSceneLayout(RTCScene sc, struct RTCB200SceneLayout* o) { SCENE_BEGIN(sc) VERIFY_HANDLE(o); scene_layout(S(sc)->gpu, o); SCENE_END }
+void rtcb200CopySceneArrays(RTCScene sc, void* nodes, void* records, struct RTCB200DescInfo* descs, unsigned int* levels, unsigned int* subs) {
+  SCENE_BEGIN(sc)
+  SceneImpl* s = S(sc);
+  const rtk::SceneGPU& g = s->gpu;
+  RTCB200SceneLayout lay;
+  scene_layout(g, &lay);
+  s->dev->use();
+  if (nodes && lay.num_nodes) cuda_check(cudaMemcpy(nodes, g.nodes, (size_t)lay.num_nodes * sizeof(rtk::Node8), cudaMemcpyDeviceToHost), "copy nodes");
+  if (records && lay.num_records) cuda_check(cudaMemcpy(records, g.tris, (size_t)lay.num_records * sizeof(rtk::TriRec), cudaMemcpyDeviceToHost), "copy records");
+  if (descs && lay.num_descs) {
+    std::vector<rtk::GeomDesc> d(lay.num_descs);
+    cuda_check(cudaMemcpy(d.data(), g.d_descs, d.size() * sizeof(rtk::GeomDesc), cudaMemcpyDeviceToHost), "copy descriptors");
+    unsigned first = 0;
+    for (size_t i = 0; i < d.size(); ++i) {
+      RTCB200DescInfo& o = descs[i];
+      o.geomID = d[i].geomID; o.instID = d[i].instID; o.kind = d[i].kind; o.first = first; o.count = d[i].ntris;
+      o.is_quad = d[i].is_quad; o.tess = d[i].tess; o.basis = d[i].basis; o.hermite = d[i].hermite;
+      memcpy(o.xfm, d[i].xfm, sizeof o.xfm);
+      first += d[i].ntris;
+    }
+  }
+  if (levels) for (unsigned l = 0; l < lay.num_levels; ++l) levels[l] = g.levels[l];
+  if (subs)
+    for (unsigned i = 0; i < lay.num_subs; ++i) {
+      subs[4 * i] = g.sub_node_off[i]; subs[4 * i + 1] = g.sub_tri_off[i];
+      subs[4 * i + 2] = g.sub_nodes[i]; subs[4 * i + 3] = g.sub_tris[i];
+    }
+  SCENE_END
+}
 void rtcb200SetSceneStatCounters(RTCScene sc, int enable) { SCENE_BEGIN(sc) S(sc)->statCounters = enable != 0; SCENE_END }
 void rtcb200ResetSceneStatCounters(RTCScene sc) { SCENE_BEGIN(sc) if (S(sc)->gpu.d_stat) { S(sc)->dev->use(); cuda_check(cudaMemset(S(sc)->gpu.d_stat, 0, 24), "reset stat counters"); } SCENE_END }
 unsigned long long rtcb200GetLaunchCount(void) { return rtk::launch_count(); }

@@ -95,6 +95,7 @@ struct SceneGPU {
   int general = 0;                      // scene has instances, quads or curves: records carry a descriptor index instead of geomID
   int curves = 0;                       // scene has curve or point records: 2 curve records among them, 1 point records only
   GeomDesc* d_descs = nullptr;          // device copy of the mesh descriptors (kept while general)
+  uint32_t num_descs = 0;               // entries of d_descs
   float bounds[6] = {0, 0, 0, 0, 0, 0};  // lower xyz, upper xyz of all valid triangles (world space, instances flattened)
   float api_bounds[6] = {0, 0, 0, 0, 0, 0};  // the same without instanced triangles
   double build_ms = 0, sah_cost = 0;

@@ -187,6 +187,15 @@ class SceneStats(C.Structure):
                 ("builder", C.c_uint), ("max_depth", C.c_uint)]
 
 
+class SceneLayout(C.Structure):
+    _fields_ = [(n, C.c_uint) for n in ("num_nodes", "num_records", "num_descs", "num_levels", "num_subs", "top_nodes", "max_depth",
+                                        "general", "robust", "builder")]
+
+
+DESC_DTYPE = np.dtype([("geomID", "<u4"), ("instID", "<u4"), ("kind", "<u4"), ("first", "<u4"), ("count", "<u4"), ("is_quad", "<u4"),
+                       ("tess", "<u4"), ("basis", "<u4"), ("hermite", "<u4"), ("xfm", "<f4", (12,))])   # RTCB200DescInfo
+
+
 def _ptr(a):
     return C.c_void_p(a.ctypes.data) if isinstance(a, np.ndarray) else C.c_void_p(a)
 
@@ -278,6 +287,8 @@ class RTCLib:
         "rtcb200GetLaunchCount": (C.c_ulonglong, []),
         "rtcb200SetTuning": (C.c_int, [C.c_char_p, C.c_int]),
         "rtcb200GetLastTraceMs": (C.c_double, [C.c_void_p]),
+        "rtcb200GetSceneLayout": (None, [C.c_void_p, C.c_void_p]),
+        "rtcb200CopySceneArrays": (None, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     }
 
     def __init__(self, path):
@@ -509,3 +520,17 @@ class RTCLib:
         s = SceneStats()
         self.rtcb200GetSceneStats(scene, C.byref(s))
         return s
+
+    def scene_arrays(self, scene):
+        """Copy of a committed scene's acceleration structure (rtcb200CopySceneArrays), for inspection: dict of the layout fields
+        and nodes (uint32 [num_nodes, 24]), records (uint32 [num_records, 12]), descs (DESC_DTYPE), levels, subs (uint32 [num_subs, 4])."""
+        lay = SceneLayout()
+        self.rtcb200GetSceneLayout(scene, C.byref(lay))
+        out = {n: getattr(lay, n) for n, _ in SceneLayout._fields_}
+        out["nodes"] = np.zeros((lay.num_nodes, 24), np.uint32)
+        out["records"] = np.zeros((lay.num_records, 12), np.uint32)
+        out["descs"] = np.zeros(lay.num_descs, DESC_DTYPE)
+        out["levels"] = np.zeros(lay.num_levels, np.uint32)
+        out["subs"] = np.zeros((lay.num_subs, 4), np.uint32)
+        self.rtcb200CopySceneArrays(scene, _ptr(out["nodes"]), _ptr(out["records"]), _ptr(out["descs"]), _ptr(out["levels"]), _ptr(out["subs"]))
+        return out

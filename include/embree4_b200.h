@@ -382,6 +382,29 @@ struct RTCB200SceneStats {
 RTCB200_API void rtcb200GetSceneStats(RTCScene scene, struct RTCB200SceneStats* out);
 RTCB200_API void rtcb200SetSceneStatCounters(RTCScene scene, int enable); /* routes queries to the counting kernel */
 RTCB200_API void rtcb200ResetSceneStatCounters(RTCScene scene);
+/* Read-only inspection of a committed scene's acceleration structure, for tests and debugging tools (no query needs it).
+ * rtcb200GetSceneLayout reports the sizes; rtcb200CopySceneArrays copies the scene's arrays into caller buffers of those sizes
+ * (any pointer may be NULL): nodes = num_nodes 96-byte BVH8 nodes, records = num_records 48-byte leaf records (layouts:
+ * embree_b200/csrc/rt_core.cuh Node8 / TriRec), descs = num_descs descriptors (general scenes -- instances, quads, curves or
+ * points -- whose records hold a descriptor index instead of a geomID), levels = num_levels node ids where each BVH8 level starts
+ * (the last entry is num_nodes; empty when the commit kept none), subs = 4 x num_subs words per mesh of a two-level scene (first
+ * node, first record, node count, record count of its relocated BVH; the first top_nodes nodes are reserved for the top level). */
+struct RTCB200SceneLayout {
+  unsigned int num_nodes, num_records, num_descs, num_levels, num_subs, top_nodes;
+  unsigned int max_depth;                /* BVH8 levels of a single-BVH build (0 for a two-level scene) */
+  unsigned int general, robust;
+  unsigned int builder;                  /* as RTCB200SceneStats.builder; 3 = two-level assembly */
+};
+struct RTCB200DescInfo {
+  unsigned int geomID, instID;           /* instID: RTC_INVALID_GEOMETRY_ID unless seen through an instance */
+  unsigned int kind;                     /* 0 triangle / quad, 1 round linear, 2 flat linear, 3 flat cubic, 4 round cubic, 5 sphere, 6 disc, 7 oriented disc point */
+  unsigned int first, count;             /* global index of the first BVH primitive, number of BVH primitives (valid or not) */
+  unsigned int is_quad, tess, basis, hermite;   /* basis: 0 Bezier, 1 B-spline, 2 Catmull-Rom (Hermite input is converted to Bezier) */
+  float xfm[12];                         /* local-to-world columns vx | vy | vz | p of the instance (identity when not instanced) */
+};
+RTCB200_API void rtcb200GetSceneLayout(RTCScene scene, struct RTCB200SceneLayout* out);
+RTCB200_API void rtcb200CopySceneArrays(RTCScene scene, void* nodes, void* records, struct RTCB200DescInfo* descs, unsigned int* levels,
+                                        unsigned int* subs);
 /* number of kernel launches issued by this library since load (bench.py's gpu_launches) */
 RTCB200_API unsigned long long rtcb200GetLaunchCount(void);
 /* experiment knobs (process-wide): kernels "collapse_policy", "c_node", "c_tri", "sah_small", "tri_batch_min",

@@ -182,6 +182,14 @@ void* emu_build(const float* verts, uint32_t nverts, const uint32_t* idx, uint32
 }
 
 void emu_free(void* h) { delete static_cast<EmuScene*>(h); }
+// copies the scene's nodes (emu_num_nodes x 96 B) and leaf records (48 B each) into `nodes` / `records` when they are not NULL;
+// returns the number of records
+uint32_t emu_export(void* h, void* nodes, void* records) {
+  const EmuScene* sc = static_cast<EmuScene*>(h);
+  if (nodes && !sc->nodes.empty()) memcpy(nodes, sc->nodes.data(), sc->nodes.size() * sizeof(Node8));
+  if (records && !sc->tris.empty()) memcpy(records, sc->tris.data(), sc->tris.size() * sizeof(TriRec));
+  return (uint32_t)sc->tris.size();
+}
 uint32_t emu_num_nodes(void* h) { return (uint32_t)static_cast<EmuScene*>(h)->nodes.size(); }
 uint32_t emu_depth(void* h) { return static_cast<EmuScene*>(h)->depth; }
 double emu_sah(void* h) { return static_cast<EmuScene*>(h)->sah; }
