@@ -18,6 +18,8 @@ RTC_FORMAT_UINT4 = 0x5004
 RTC_FORMAT_FLOAT3 = 0x9003
 RTC_BUFFER_TYPE_INDEX = 0
 RTC_BUFFER_TYPE_VERTEX = 1
+RTC_BUFFER_TYPE_VERTEX_ATTRIBUTE = 2
+RTC_FORMAT_FLOAT = 0x9001   # RTC_FORMAT_FLOAT2 .. RTC_FORMAT_FLOAT16 follow
 RTC_GEOMETRY_TYPE_TRIANGLE = 0
 RTC_GEOMETRY_TYPE_QUAD = 1
 RTC_GEOMETRY_TYPE_ROUND_LINEAR_CURVE = 16
@@ -175,6 +177,23 @@ class InterpolateArguments(C.Structure):
                 ("valueCount", C.c_uint)]
 
 
+class InterpolateNArguments(C.Structure):
+    """RTCInterpolateNArguments (rtcore_geometry.h:318-337)."""
+    _fields_ = [("geometry", C.c_void_p), ("valid", C.c_void_p), ("primIDs", C.c_void_p), ("u", C.c_void_p), ("v", C.c_void_p), ("N", C.c_uint),
+                ("bufferType", C.c_int), ("bufferSlot", C.c_uint), ("P", C.c_void_p), ("dPdu", C.c_void_p), ("dPdv", C.c_void_p),
+                ("ddPdudu", C.c_void_p), ("ddPdvdv", C.c_void_p), ("ddPdudv", C.c_void_p), ("valueCount", C.c_uint)]
+
+
+class InterpolateHitsArguments(C.Structure):
+    """RTCB200InterpolateHitsArguments (include/embree4_b200.h, Section B)."""
+    _fields_ = [("hits", C.c_void_p), ("M", C.c_size_t), ("bufferType", C.c_int), ("bufferSlot", C.c_uint), ("valueCount", C.c_uint),
+                ("P", C.c_void_p), ("dPdu", C.c_void_p), ("dPdv", C.c_void_p), ("ddPdudu", C.c_void_p), ("ddPdvdv", C.c_void_p),
+                ("ddPdudv", C.c_void_p)]
+
+
+INTERP_OUTPUTS = ("P", "dPdu", "dPdv", "ddPdudu", "ddPdvdv", "ddPdudv")
+
+
 class RTCBounds(C.Structure):
     _fields_ = [(n, C.c_float) for n in
                 ("lower_x", "lower_y", "lower_z", "align0", "upper_x", "upper_y", "upper_z", "align1")]
@@ -234,6 +253,7 @@ class RTCLib:
         "rtcUpdateGeometryBuffer": (None, [C.c_void_p, C.c_int, C.c_uint]),
         "rtcSetGeometryTessellationRate": (None, [C.c_void_p, C.c_float]),
         "rtcInterpolate": (None, [C.c_void_p]),
+        "rtcInterpolateN": (None, [C.c_void_p]),
         "rtcSetGeometryUserData": (None, [C.c_void_p, C.c_void_p]),
         "rtcGetGeometryUserData": (C.c_void_p, [C.c_void_p]),
         "rtcSetGeometryIntersectFilterFunction": (None, [C.c_void_p, C.c_void_p]),
@@ -289,6 +309,8 @@ class RTCLib:
         "rtcb200GetLastTraceMs": (C.c_double, [C.c_void_p]),
         "rtcb200GetSceneLayout": (None, [C.c_void_p, C.c_void_p]),
         "rtcb200CopySceneArrays": (None, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+        "rtcb200InterpolateHits": (None, [C.c_void_p, C.c_void_p]),
+        "rtcb200InterpolateHitsDevice": (None, [C.c_void_p, C.c_void_p, C.c_void_p]),
     }
 
     def __init__(self, path):
@@ -534,3 +556,27 @@ class RTCLib:
         out["subs"] = np.zeros((lay.num_subs, 4), np.uint32)
         self.rtcb200CopySceneArrays(scene, _ptr(out["nodes"]), _ptr(out["records"]), _ptr(out["descs"]), _ptr(out["levels"]), _ptr(out["subs"]))
         return out
+
+    def interpolate_hits(self, scene, hits, buffer_type, slot, value_count, want=("P", "dPdu", "dPdv"), stream=None, out=None):
+        """rtcb200InterpolateHits* of `hits`: a structured numpy array of RAYHIT_DTYPE (host variant) or a CUDA tensor holding M
+        RTCRayHit records (96 bytes each; device variant, enqueued on `stream`, a torch.cuda.Stream or None for the current one).
+        `want` names the outputs (INTERP_OUTPUTS; dPdu comes with dPdv, ddPdudu with ddPdvdv and ddPdudv).  Returns {name: [value_count, M]
+        float32 array or tensor}; `out` may pass those arrays in (a miss leaves its entries as they were), otherwise they start as NaN."""
+        a = InterpolateHitsArguments()
+        a.bufferType, a.bufferSlot, a.valueCount = buffer_type, slot, value_count
+        if isinstance(hits, np.ndarray):
+            a.hits, a.M = hits.ctypes.data, len(hits)
+            res = out if out is not None else {n: np.full((value_count, len(hits)), np.nan, np.float32) for n in want}
+            for n in want:
+                setattr(a, n, res[n].ctypes.data)
+            self.rtcb200InterpolateHits(scene, C.byref(a))
+            return res
+        import torch
+        M = hits.numel() * hits.element_size() // 96
+        a.hits, a.M = hits.data_ptr(), M
+        res = out if out is not None else {n: torch.full((value_count, M), float("nan"), dtype=torch.float32, device=hits.device) for n in want}
+        for n in want:
+            setattr(a, n, res[n].data_ptr())
+        st = stream if stream is not None else torch.cuda.current_stream(hits.device)
+        self.rtcb200InterpolateHitsDevice(scene, C.byref(a), C.c_void_p(st.cuda_stream))
+        return res
