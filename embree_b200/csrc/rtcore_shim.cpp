@@ -1726,6 +1726,24 @@ void rtcb200GetSceneStats(RTCScene sc, struct RTCB200SceneStats* o) {
   }
   SCENE_END
 }
+// the arrays trace_device hands the kernel (make_params), for device-side queries; refused where trace_device would refuse
+void rtcb200GetSceneDeviceTraversable(RTCScene sc, struct RTCB200DeviceTraversable* o) {
+  SCENE_BEGIN(sc)
+  VERIFY_HANDLE(o);
+  memset(o, 0, sizeof *o);
+  SceneImpl* s = S(sc);
+  std::lock_guard<std::mutex> lk(s->commitMutex);
+  if (!s->everCommitted) fail(RTC_ERROR_INVALID_OPERATION, "Traversable is NULL. The scene has to be committed first.");
+  const QueryArgs none;   // no arguments' filter: only the geometries' own callbacks count
+  if (filters_apply(s, none, 0) || filters_apply(s, none, 1))
+    fail(RTC_ERROR_INVALID_OPERATION, "filter callbacks are host functions: device-side queries cannot call them");
+  const rtk::SceneGPU& g = s->gpu;
+  o->nodes = g.nodes; o->records = g.tris;
+  o->descs = g.general ? g.d_descs : nullptr;
+  o->root_valid = g.root_valid; o->robust = (unsigned)g.robust; o->general = (unsigned)g.general; o->curves = (unsigned)g.curves;
+  o->device = s->dev->gpu;
+  SCENE_END
+}
 static void scene_layout(const rtk::SceneGPU& g, RTCB200SceneLayout* o) {
   memset(o, 0, sizeof *o);
   if (g.root_valid) {

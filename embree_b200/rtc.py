@@ -211,6 +211,13 @@ class SceneLayout(C.Structure):
                                         "general", "robust", "builder")]
 
 
+class DeviceTraversable(C.Structure):
+    """RTCB200DeviceTraversable (include/embree4_b200.h, Section B): a committed scene's device arrays, passed by value to kernels
+    that trace with include/embree4_b200_device.cuh."""
+    _fields_ = [("nodes", C.c_void_p), ("records", C.c_void_p), ("descs", C.c_void_p), ("root_valid", C.c_uint), ("robust", C.c_uint),
+                ("general", C.c_uint), ("curves", C.c_uint), ("device", C.c_int)]
+
+
 DESC_DTYPE = np.dtype([("geomID", "<u4"), ("instID", "<u4"), ("kind", "<u4"), ("first", "<u4"), ("count", "<u4"), ("is_quad", "<u4"),
                        ("tess", "<u4"), ("basis", "<u4"), ("hermite", "<u4"), ("xfm", "<f4", (12,))])   # RTCB200DescInfo
 
@@ -311,6 +318,7 @@ class RTCLib:
         "rtcb200CopySceneArrays": (None, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
         "rtcb200InterpolateHits": (None, [C.c_void_p, C.c_void_p]),
         "rtcb200InterpolateHitsDevice": (None, [C.c_void_p, C.c_void_p, C.c_void_p]),
+        "rtcb200GetSceneDeviceTraversable": (None, [C.c_void_p, C.c_void_p]),
     }
 
     def __init__(self, path):
@@ -542,6 +550,13 @@ class RTCLib:
         s = SceneStats()
         self.rtcb200GetSceneStats(scene, C.byref(s))
         return s
+
+    def scene_device_traversable(self, scene):
+        """rtcb200GetSceneDeviceTraversable: the DeviceTraversable of a committed scene (all zero, with the error recorded, when
+        the scene is refused)."""
+        t = DeviceTraversable()
+        self.rtcb200GetSceneDeviceTraversable(scene, C.byref(t))
+        return t
 
     def scene_arrays(self, scene):
         """Copy of a committed scene's acceleration structure (rtcb200CopySceneArrays), for inspection: dict of the layout fields

@@ -450,6 +450,27 @@ struct RTCB200InterpolateHitsArguments {
 RTCB200_API void rtcb200InterpolateHits(RTCScene scene, const struct RTCB200InterpolateHitsArguments* args);
 RTCB200_API void rtcb200InterpolateHitsDevice(RTCScene scene, const struct RTCB200InterpolateHitsArguments* args, void* cuda_stream);
 
+/* Tracing from the caller's own CUDA kernels (what rtcTraversableIntersect1 / rtcTraversableOccluded1 are in Embree 4's SYCL
+ * device code, rtcore_scene.h:266,304).  rtcb200GetSceneDeviceTraversable fills `out` with the device arrays of a committed
+ * scene; the struct is passed to a kernel by value, where include/embree4_b200_device.cuh's rtcb200TraversableIntersect1 /
+ * rtcb200TraversableOccluded1 trace one ray per call, with the results of rtcb200Intersect1MDevice / rtcb200Occluded1MDevice.
+ *  - Refused, with RTC_ERROR_INVALID_OPERATION recorded and `*out` zeroed: a scene that was never committed, and a scene in which
+ *    an enabled geometry -- its own or one of a scene it instances -- has an intersect or occluded filter function (filters are
+ *    host functions).  rtcSetGeometryEnableFilterFunctionFromArguments alone is accepted: no filter is ever called on the device.
+ *  - Valid until the scene's next rtcCommitScene or its final release: kernels that use it must have completed before either.
+ *  - Use it on the scene's CUDA device (`device`).  Its fields are not part of the interface. */
+struct RTCB200DeviceTraversable {
+  const void* nodes;         /* BVH8 nodes */
+  const void* records;       /* leaf records */
+  const void* descs;         /* per-geometry descriptors of a scene with instances, quads, curves or points; NULL otherwise */
+  unsigned int root_valid;   /* 0: empty scene */
+  unsigned int robust;       /* RTC_SCENE_FLAG_ROBUST */
+  unsigned int general;      /* records index `descs` */
+  unsigned int curves;       /* 2: curve records among them, 1: point records only */
+  int device;                /* CUDA ordinal of the scene's device */
+};
+RTCB200_API void rtcb200GetSceneDeviceTraversable(RTCScene scene, struct RTCB200DeviceTraversable* out);
+
 /* =====================================================================================================
  * Section C -- the rest of the reference library's export list (kernels/export.linux.map: every rtc* symbol).
  * Thin variants of supported calls and rtcInterpolate / rtcInterpolateN are implemented; the others (user and subdivision
