@@ -229,6 +229,16 @@ struct SceneImpl : RefCounted {
   // copies of the buffers it reads; built by the first call that needs it, freed by the next commit and with the scene
   struct InterpTable { RTCBufferType type; unsigned slot; rtk::InterpEntry* d_table; uint32_t nentries; std::vector<void*> buffers; };
   std::vector<InterpTable> interpTables;
+  // device-side argument filters (rtcb200GetSceneDeviceTraversable): (geomID, instID or invalid) of every descriptor of the last
+  // commit, and the {userPtr, argFilterEnabled} snapshots the getter uploaded since then -- the newest is reused while it is
+  // unchanged; the next commit frees them all, and so does releasing the scene
+  std::vector<std::pair<uint32_t, uint32_t>> descIds;
+  std::vector<void*> geomTables;
+  std::vector<RTCB200DeviceGeometry> lastGeomTable;
+  void free_geom_tables() {
+    for (void* p : geomTables) cudaFreeAsync(p, 0);
+    geomTables.clear(); lastGeomTable.clear();
+  }
   void free_interp() {
     for (InterpTable& t : interpTables) {
       cudaFreeAsync(t.d_table, 0);
@@ -255,6 +265,7 @@ struct SceneImpl : RefCounted {
     for (void* p : deviceBuffers) cudaFreeAsync(p, 0);
     for (void* p : residentBuffers) cudaFreeAsync(p, 0);
     free_interp();
+    free_geom_tables();
     free_subs();
     rtk::free_scene(gpu);
     if (ev0) cudaEventDestroy(ev0);
@@ -645,6 +656,8 @@ void commit_single(SceneImpl* s, const std::vector<GeometryImpl*>& geoms, bool t
     rtk::free_scene(s->gpu);
     build_failed(r, errmsg);
   }
+  if (s->gpu.general)   // the build uploads the descriptors in this order (rtk::SceneGPU::d_descs)
+    for (const rtk::GeomDesc& d : up.descs) s->descIds.push_back({d.geomID, d.has_xfm ? d.instID : RTC_INVALID_GEOMETRY_ID});
   for (int a = 0; a < 3; ++a) {   // rtcGetSceneBounds: own triangles + instance boxes
     s->apiBounds[a] = fminf(s->gpu.api_bounds[a], instBounds[a]);
     s->apiBounds[3 + a] = fmaxf(s->gpu.api_bounds[3 + a], instBounds[3 + a]);
@@ -673,6 +686,8 @@ void commit_scene(SceneImpl* s) {
   release_buffers(s->residentBuffers);
   s->residentCurves.clear();
   s->free_interp();
+  s->free_geom_tables();
+  s->descIds.clear();
   const TwoLevelChoice twoLevel = choose_two_level(s, geoms);
   if (twoLevel.chosen) commit_two_level(s, geoms);
   else commit_single(s, geoms, twoLevel.possible);
@@ -1726,6 +1741,52 @@ void rtcb200GetSceneStats(RTCScene sc, struct RTCB200SceneStats* o) {
   }
   SCENE_END
 }
+// What the device-side argument filters read about the geometry of a record (embree4_b200.h RTCB200DeviceGeometry), one entry per
+// value of a record's b.w: the geomID in a triangle-only scene, the descriptor index otherwise, an instanced descriptor taking its
+// child geometry's values -- the geometry hit_geometry() finds for the host-pointer path.  User data and the filter switch change
+// without a commit, so every call takes them anew; an unchanged table is not uploaded twice.  Called with commitMutex held.
+static const RTCB200DeviceGeometry* geometry_snapshot(SceneImpl* s) {
+  std::vector<RTCB200DeviceGeometry> tab;
+  auto entry = [](const GeometryImpl* g) {
+    RTCB200DeviceGeometry e;
+    memset(&e, 0, sizeof e);
+    if (g) { e.userPtr = g->userPtr; e.argFilterEnabled = g->argFilterEnabled ? 1u : 0u; }
+    return e;
+  };
+  {
+    std::lock_guard<std::mutex> lg(s->geomMutex);
+    if (!s->gpu.general) {
+      for (const GeometryImpl* g : s->geoms) tab.push_back(entry(g));
+    } else {
+      for (const auto& id : s->descIds) {
+        const GeometryImpl* g = nullptr;
+        if (id.second == RTC_INVALID_GEOMETRY_ID) g = id.first < s->geoms.size() ? s->geoms[id.first] : nullptr;
+        else if (id.second < s->geoms.size() && s->geoms[id.second] && s->geoms[id.second]->instScene) {
+          SceneImpl* c = s->geoms[id.second]->instScene;
+          std::lock_guard<std::mutex> lc(c->geomMutex);
+          g = id.first < c->geoms.size() ? c->geoms[id.first] : nullptr;
+        }
+        tab.push_back(entry(g));
+      }
+    }
+  }
+  if (tab.empty()) tab.push_back(entry(nullptr));
+  const size_t bytes = tab.size() * sizeof(RTCB200DeviceGeometry);
+  if (!s->geomTables.empty() && tab.size() == s->lastGeomTable.size() && memcmp(tab.data(), s->lastGeomTable.data(), bytes) == 0)
+    return static_cast<const RTCB200DeviceGeometry*>(s->geomTables.back());
+  // on the calling thread's own non-blocking stream: the upload waits for no other work, and is complete when the getter returns
+  // (the caller's kernels run on streams of their own)
+  s->dev->use();
+  t_ctx.ensure(s->dev->gpu);
+  void* p = nullptr;
+  cuda_check(cudaMallocAsync(&p, bytes, t_ctx.stream), "cudaMallocAsync(geometry table)");
+  s->geomTables.push_back(p);
+  cuda_check(cudaMemcpyAsync(p, tab.data(), bytes, cudaMemcpyHostToDevice, t_ctx.stream), "upload geometry table");
+  cuda_check(cudaStreamSynchronize(t_ctx.stream), "upload geometry table");
+  s->lastGeomTable.swap(tab);
+  return static_cast<const RTCB200DeviceGeometry*>(p);
+}
+
 // the arrays trace_device hands the kernel (make_params), for device-side queries; refused where trace_device would refuse
 void rtcb200GetSceneDeviceTraversable(RTCScene sc, struct RTCB200DeviceTraversable* o) {
   SCENE_BEGIN(sc)
@@ -1738,10 +1799,12 @@ void rtcb200GetSceneDeviceTraversable(RTCScene sc, struct RTCB200DeviceTraversab
   if (filters_apply(s, none, 0) || filters_apply(s, none, 1))
     fail(RTC_ERROR_INVALID_OPERATION, "filter callbacks are host functions: device-side queries cannot call them");
   const rtk::SceneGPU& g = s->gpu;
+  const RTCB200DeviceGeometry* geoms = g.root_valid ? geometry_snapshot(s) : nullptr;
   o->nodes = g.nodes; o->records = g.tris;
   o->descs = g.general ? g.d_descs : nullptr;
-  o->root_valid = g.root_valid; o->robust = (unsigned)g.robust; o->general = (unsigned)g.general; o->curves = (unsigned)g.curves;
-  o->device = s->dev->gpu;
+  o->root_valid = g.root_valid; o->robust = (unsigned)g.robust; o->general = (unsigned short)g.general; o->curves = (unsigned)g.curves;
+  o->device = (short)s->dev->gpu;
+  o->geometries = geoms;
   SCENE_END
 }
 static void scene_layout(const rtk::SceneGPU& g, RTCB200SceneLayout* o) {

@@ -44,6 +44,9 @@ RTC_SCENE_FLAG_NONE, RTC_SCENE_FLAG_DYNAMIC, RTC_SCENE_FLAG_COMPACT, RTC_SCENE_F
 RTC_RAY_QUERY_FLAG_INCOHERENT = 0
 RTC_RAY_QUERY_FLAG_COHERENT = 1 << 16
 RTC_FEATURE_FLAG_ALL = 0xFFFFFFFF
+RTC_FEATURE_FLAG_FILTER_FUNCTION_IN_ARGUMENTS = 1 << 24
+RTC_FEATURE_FLAG_FILTER_FUNCTION_IN_GEOMETRY = 1 << 25
+RTC_FEATURE_FLAG_FILTER_FUNCTION = RTC_FEATURE_FLAG_FILTER_FUNCTION_IN_ARGUMENTS | RTC_FEATURE_FLAG_FILTER_FUNCTION_IN_GEOMETRY
 RTC_ERROR_NONE, RTC_ERROR_UNKNOWN, RTC_ERROR_INVALID_ARGUMENT, RTC_ERROR_INVALID_OPERATION = 0, 1, 2, 3
 
 # numpy views of the I/O records ---------------------------------------------------------------
@@ -215,7 +218,12 @@ class DeviceTraversable(C.Structure):
     """RTCB200DeviceTraversable (include/embree4_b200.h, Section B): a committed scene's device arrays, passed by value to kernels
     that trace with include/embree4_b200_device.cuh."""
     _fields_ = [("nodes", C.c_void_p), ("records", C.c_void_p), ("descs", C.c_void_p), ("root_valid", C.c_uint), ("robust", C.c_uint),
-                ("general", C.c_uint), ("curves", C.c_uint), ("device", C.c_int)]
+                ("general", C.c_ushort), ("device", C.c_short), ("curves", C.c_uint), ("geometries", C.c_void_p)]
+
+
+class DeviceGeometry(C.Structure):
+    """RTCB200DeviceGeometry: one entry of DeviceTraversable.geometries, what device-side argument filters read of a geometry."""
+    _fields_ = [("userPtr", C.c_void_p), ("argFilterEnabled", C.c_uint)]
 
 
 DESC_DTYPE = np.dtype([("geomID", "<u4"), ("instID", "<u4"), ("kind", "<u4"), ("first", "<u4"), ("count", "<u4"), ("is_quad", "<u4"),

@@ -31,6 +31,12 @@ extern "C" {
 #define RTCB200_ALIGN(n)
 #define RTCB200_API
 #endif
+/* the rtcInit* helpers below also run in device code (kernels that trace with embree4_b200_device.cuh) */
+#if defined(__CUDACC__)
+#define RTCB200_HD __host__ __device__
+#else
+#define RTCB200_HD
+#endif
 
 /* ---- version / constants (kernels/rtcore_config.h.in:10-16, rtcore_common.h:51-54) ---- */
 #define RTC_VERSION_MAJOR 4
@@ -91,6 +97,8 @@ enum RTCFeatureFlags {
   RTC_FEATURE_FLAG_FLAT_HERMITE_CURVE = 1 << 15, RTC_FEATURE_FLAG_FLAT_CATMULL_ROM_CURVE = 1 << 18,
   RTC_FEATURE_FLAG_SPHERE_POINT = 1 << 20, RTC_FEATURE_FLAG_DISC_POINT = 1 << 21, RTC_FEATURE_FLAG_ORIENTED_DISC_POINT = 1 << 22,
   RTC_FEATURE_FLAG_INSTANCE = 1 << 23,
+  RTC_FEATURE_FLAG_FILTER_FUNCTION_IN_ARGUMENTS = 1 << 24, RTC_FEATURE_FLAG_FILTER_FUNCTION_IN_GEOMETRY = 1 << 25,
+  RTC_FEATURE_FLAG_FILTER_FUNCTION = RTC_FEATURE_FLAG_FILTER_FUNCTION_IN_ARGUMENTS | RTC_FEATURE_FLAG_FILTER_FUNCTION_IN_GEOMETRY,
   RTC_FEATURE_FLAG_ALL = 0xffffffff
 };
 enum RTCGeometryType {
@@ -180,8 +188,9 @@ struct RTCB200_ALIGN(16) RTCBounds { /* rtcore_common.h:163-167 */
 struct RTCB200_ALIGN(16) RTCLinearBounds { struct RTCBounds bounds0, bounds1; };
 
 /* per-query context and arguments (rtcore_common.h:335-361, rtcore_scene.h:34-86).  `filter` is honoured by the
- * host-pointer entry points (see below); the Device entry points cannot call back into the host and record
- * RTC_ERROR_INVALID_OPERATION when a filter applies.  `intersect`/`occluded` (user geometries) must be NULL. */
+ * host-pointer entry points (see below) and, as a __device__ function, by the device-side queries of
+ * embree4_b200_device.cuh; the batched Device entry points cannot call it and record RTC_ERROR_INVALID_OPERATION when a
+ * filter applies.  `intersect`/`occluded` (user geometries) must be NULL. */
 struct RTCRayQueryContext {
   unsigned int instID[RTC_MAX_INSTANCE_LEVEL_COUNT];
   unsigned int instPrimID[RTC_MAX_INSTANCE_LEVEL_COUNT];
@@ -189,7 +198,8 @@ struct RTCRayQueryContext {
 /* Filter callbacks (rtcore_common.h:311-324): called on the HOST for every candidate hit of a geometry that has a filter
  * (or, with RTC_RAY_QUERY_FLAG_INVOKE_ARGUMENT_FILTER / rtcSetGeometryEnableFilterFunctionFromArguments, for the
  * arguments' filter), always with N == 1: `ray` is an RTCRay whose tfar is the candidate distance, `hit` an RTCHit.
- * Setting valid[0] = 0 rejects the hit and the traversal goes on without it.  Host-pointer entry points only. */
+ * Setting valid[0] = 0 rejects the hit and the traversal goes on without it.  Host-pointer entry points, and the device-side
+ * queries of embree4_b200_device.cuh with a __device__ function as the arguments' filter. */
 struct RTCRayN;
 struct RTCHitN;
 struct RTCFilterFunctionNArguments {
@@ -206,14 +216,14 @@ struct RTCOccludedArguments {
   enum RTCRayQueryFlags flags; enum RTCFeatureFlags feature_mask; struct RTCRayQueryContext* context;
   RTCFilterFunctionN filter; RTCOccludedFunctionN occluded;
 };
-static inline void rtcInitRayQueryContext(struct RTCRayQueryContext* c) {
+static inline RTCB200_HD void rtcInitRayQueryContext(struct RTCRayQueryContext* c) {
   c->instID[0] = RTC_INVALID_GEOMETRY_ID; c->instPrimID[0] = RTC_INVALID_GEOMETRY_ID;
 }
-static inline void rtcInitIntersectArguments(struct RTCIntersectArguments* a) {
+static inline RTCB200_HD void rtcInitIntersectArguments(struct RTCIntersectArguments* a) {
   a->flags = RTC_RAY_QUERY_FLAG_INCOHERENT; a->feature_mask = RTC_FEATURE_FLAG_ALL; a->context = NULL;
   a->filter = NULL; a->intersect = NULL;
 }
-static inline void rtcInitOccludedArguments(struct RTCOccludedArguments* a) {
+static inline RTCB200_HD void rtcInitOccludedArguments(struct RTCOccludedArguments* a) {
   a->flags = RTC_RAY_QUERY_FLAG_INCOHERENT; a->feature_mask = RTC_FEATURE_FLAG_ALL; a->context = NULL;
   a->filter = NULL; a->occluded = NULL;
 }
@@ -455,20 +465,32 @@ RTCB200_API void rtcb200InterpolateHitsDevice(RTCScene scene, const struct RTCB2
  * scene; the struct is passed to a kernel by value, where include/embree4_b200_device.cuh's rtcb200TraversableIntersect1 /
  * rtcb200TraversableOccluded1 trace one ray per call, with the results of rtcb200Intersect1MDevice / rtcb200Occluded1MDevice.
  *  - Refused, with RTC_ERROR_INVALID_OPERATION recorded and `*out` zeroed: a scene that was never committed, and a scene in which
- *    an enabled geometry -- its own or one of a scene it instances -- has an intersect or occluded filter function (filters are
- *    host functions).  rtcSetGeometryEnableFilterFunctionFromArguments alone is accepted: no filter is ever called on the device.
+ *    an enabled geometry -- its own or one of a scene it instances -- has an intersect or occluded filter function (geometry
+ *    filters are host functions; Embree 4 does not run them on a GPU either).  rtcSetGeometryEnableFilterFunctionFromArguments
+ *    is accepted: device-side queries that opt in to filters call the arguments' filter (RTCIntersectArguments::filter) for them.
+ *  - Each call snapshots every geometry's user data and argument-filter switch (`geometries`, read by those filters): a later
+ *    rtcSetGeometryUserData or rtcSetGeometryEnableFilterFunctionFromArguments shows in the traversable of a later call, never
+ *    in one already taken.  A call on an unchanged scene reuses its last snapshot.  A call that uploads one waits for that upload
+ *    (on a stream of the calling thread's own), not for other work.  Only kernels that opt in to argument filters
+ *    (rtcb200TraversableIntersect1<RTC_FEATURE_FLAG_FILTER_FUNCTION_IN_ARGUMENTS>, embree4_b200_device.cuh) read it.
  *  - Valid until the scene's next rtcCommitScene or its final release: kernels that use it must have completed before either.
  *  - Use it on the scene's CUDA device (`device`).  Its fields are not part of the interface. */
+struct RTCB200DeviceGeometry {
+  void* userPtr;                   /* rtcSetGeometryUserData of the geometry (of the instanced child, through an instance) */
+  unsigned int argFilterEnabled;   /* rtcSetGeometryEnableFilterFunctionFromArguments */
+};
 struct RTCB200DeviceTraversable {
   const void* nodes;         /* BVH8 nodes */
   const void* records;       /* leaf records */
   const void* descs;         /* per-geometry descriptors of a scene with instances, quads, curves or points; NULL otherwise */
   unsigned int root_valid;   /* 0: empty scene */
   unsigned int robust;       /* RTC_SCENE_FLAG_ROBUST */
-  unsigned int general;      /* records index `descs` */
+  unsigned short general;    /* records index `descs` */
+  short device;              /* CUDA ordinal of the scene's device */
   unsigned int curves;       /* 2: curve records among them, 1: point records only */
-  int device;                /* CUDA ordinal of the scene's device */
-};
+  const struct RTCB200DeviceGeometry* geometries;   /* indexed like `descs` (by geomID when `descs` is NULL); NULL: empty scene */
+};   /* 48 bytes, the fields the queries read at fixed offsets: kernels take the struct by value, and a larger parameter would
+      change the code of every kernel that traces, filters or not */
 RTCB200_API void rtcb200GetSceneDeviceTraversable(RTCScene scene, struct RTCB200DeviceTraversable* out);
 
 /* =====================================================================================================

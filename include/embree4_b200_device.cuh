@@ -16,22 +16,142 @@
 // are written (tfar, Ng, u, v, primID, geomID, instID[0], instPrimID[0]; occluded: tfar = -inf), a miss leaves the record
 // untouched, a ray with tfar < 0 counts as already occluded and an empty scene returns at once.
 //
-// `args` may be NULL or point to memory the calling thread can read.  Only args->context is read: its instID[0] and
-// instPrimID[0] seed a hit's instance ids, as on the host.  args->filter, flags and feature_mask are ignored -- no filter runs
-// on the device, and the scene's statistics counters do not count these queries.
+// `args` may be NULL or point to memory the calling thread can read.  args->context's instID[0] and instPrimID[0] seed a hit's
+// instance ids, as on the host.  The scene's statistics counters do not count these queries.
+//
+// Argument filters (Embree 4's filter_sycl.h: on a GPU only the filter passed in the arguments runs).  A kernel opts in at compile
+// time, as Embree 4's SYCL feature-mask specialisation does: rtcb200TraversableIntersect1<FEATURES> / Occluded1<FEATURES> with
+// RTC_FEATURE_FLAG_FILTER_FUNCTION_IN_ARGUMENTS in FEATURES.  The calls without a template argument compile no filter code, ignore
+// args->filter and cost a kernel nothing.  In an opted-in call, when args->filter is set and args->feature_mask has
+// RTC_FEATURE_FLAG_FILTER_FUNCTION_IN_ARGUMENTS, every candidate that passes the primitive test is offered to the filter if its
+// geometry -- the instanced child, through an instance -- enabled it with rtcSetGeometryEnableFilterFunctionFromArguments, or if
+// args->flags has RTC_RAY_QUERY_FLAG_INVOKE_ARGUMENT_FILTER:
+//
+//   __device__ void cutout(const RTCFilterFunctionNArguments* a) {      // N == 1
+//     const RTCHit* h = (const RTCHit*)a->hit;
+//     if (alpha(a->geometryUserPtr, h->primID, h->u, h->v) < 0.5f) a->valid[0] = 0;
+//   }
+//   __global__ void shade(RTCB200DeviceTraversable t, ...) {
+//     RTCIntersectArguments args; rtcInitIntersectArguments(&args);
+//     args.filter = cutout;                    // the address is taken in DEVICE code (or read from a __device__ variable)
+//     rtcb200TraversableIntersect1<RTC_FEATURE_FLAG_FILTER_FUNCTION_IN_ARGUMENTS>(t, &rh, &args);
+//   }
+//
+//  - The opted-in kernel holds both the filtered and the unfiltered variants: more registers, whether a filter runs or not.
+//  - The filter must be a __device__ function: a host function's address cannot be called here.  Without -rdc it has to live in
+//    the translation unit of the kernel; with -rdc=true anywhere in the device link.
+//  - Each call gets N = 1, valid[0] = -1, the geometry's user data (as rtcb200GetSceneDeviceTraversable snapshot it), `context` =
+//    args->context (a default one in the thread's memory when NULL), `ray` = a copy of the caller's world-space RTCRay with tfar =
+//    the candidate's t, and `hit` = the RTCHit the candidate would be written as.  During the call context->instID[0] /
+//    instPrimID[0] hold the candidate's instance ids; they are restored afterwards, so a context shared by several threads races.
+//  - Accepted (valid[0] != 0): closest hit -- the candidate becomes the hit, written as the filter left `hit`, and the `ray.tfar`
+//    it left is the distance further candidates are culled against; any hit -- the query writes tfar = -inf and returns.
+//    Rejected: nothing changes and traversal goes on; that record is not offered to this ray again.
+//  - Candidates come in traversal order, one per leaf record (a sphere point's back hit, or a second root of a curve segment,
+//    is not offered after its front hit is rejected).  Geometry filter callbacks never run on the device.
+//  - The scene flag RTC_SCENE_FLAG_FILTER_FUNCTION_IN_ARGUMENTS is not required, as on the host.
 #pragma once
 #include "embree4_b200.h"
 #include "../embree_b200/csrc/record_tests.cuh"
 
 namespace rtk {
 
+
 // One query of one thread, specialised as the batched kernel is (trace.cu launch_k): GENERAL 0 = triangle records with
 // geomIDs, 1 = records through descriptors (instances, quads), 2 = with curve or point records; ROBUST = Pluecker test.
 // The record test and the write-back restate trace.cu's test_tri and write_back for one lane (the tests of
 // tests/test_device_traversal.py compare both bit for bit); closest-hit triangle scenes follow the SPREAD instantiation's
 // acceptance rule, which is what the batched entry points run there.
+// trace.cu write_back for one record: the RTCHit of record `ti` hit at (u, v) by the world-space ray r0 -- a curve / point
+// record with the normal its test kept (cng*).  Ng stays in object space.
+template <bool ROBUST, int GENERAL>
+__device__ __forceinline__ void record_hit(const uint4* __restrict__ recs, const GeomDesc* __restrict__ descs, uint32_t ti, const Ray& r0, float u,
+                                           float v, float cngx, float cngy, float cngz, uint32_t instID, uint32_t instPrimID, RTCHit& h) {
+  const uint4* tp = recs + (size_t)ti * 3;
+  const uint4 a = __ldg(tp), b = __ldg(tp + 1), c = __ldg(tp + 2);
+  float ngx, ngy, ngz;
+  uint32_t primID = a.w, geomID = b.w;
+  float lox = r0.ox, loy = r0.oy, loz = r0.oz;   // ray origin in the space the record's triangle lives in
+  bool curve_hit = false;
+  if (GENERAL) {
+    const GeomDesc& d = descs[b.w];
+    geomID = d.geomID;
+    if (GENERAL == 2 && d.kind != PRIM_TRIANGLE) { ngx = cngx; ngy = cngy; ngz = cngz; curve_hit = true; }
+    if (d.has_xfm) {
+      instID = d.instID; instPrimID = 0u;   // instance_id_stack::push(context, instID, 0)
+      if (ROBUST) { Ray lr = r0; to_object_space(d, lr); lox = lr.ox; loy = lr.oy; loz = lr.oz; }
+    }
+  }
+  if (curve_hit) {
+  } else if (ROBUST) {   // stable_triangle_normal of the origin-relative edges, exactly as in tri_test_pluecker
+    const float v0x = sub_rn(__uint_as_float(a.x), lox), v0y = sub_rn(__uint_as_float(a.y), loy), v0z = sub_rn(__uint_as_float(a.z), loz);
+    const float v1x = sub_rn(__uint_as_float(b.x), lox), v1y = sub_rn(__uint_as_float(b.y), loy), v1z = sub_rn(__uint_as_float(b.z), loz);
+    const float v2x = sub_rn(__uint_as_float(c.x), lox), v2y = sub_rn(__uint_as_float(c.y), loy), v2z = sub_rn(__uint_as_float(c.z), loz);
+    stable_normal(sub_rn(v2x, v0x), sub_rn(v2y, v0y), sub_rn(v2z, v0z), sub_rn(v0x, v1x), sub_rn(v0y, v1y), sub_rn(v0z, v1z),
+                  sub_rn(v1x, v2x), sub_rn(v1y, v2y), sub_rn(v1z, v2z), ngx, ngy, ngz);
+  } else {
+    const float e1x = __uint_as_float(b.x), e1y = __uint_as_float(b.y), e1z = __uint_as_float(b.z);
+    const float e2x = __uint_as_float(c.x), e2y = __uint_as_float(c.y), e2z = __uint_as_float(c.z);
+    ngx = msub(e2y, e1z, mul_rn(e2z, e1y));
+    ngy = msub(e2z, e1x, mul_rn(e2x, e1z));
+    ngz = msub(e2x, e1y, mul_rn(e2y, e1x));
+  }
+  if (GENERAL && !curve_hit && (a.w >> 31)) {   // quad halves share the quad's primID; the second one has flipped winding
+    primID = a.w & 0x7FFFFFFFu;
+    ngx = -ngx; ngy = -ngy; ngz = -ngz;
+  }
+  h.Ng_x = ngx; h.Ng_y = ngy; h.Ng_z = ngz; h.u = u; h.v = v;
+  h.primID = primID; h.geomID = geomID; h.instID[0] = instID; h.instPrimID[0] = instPrimID;
+}
+
+// A filtered query's state in the thread's local memory: the traversal loop keeps only its address, so the filtered variants
+// hold about as many registers as the others and the caller's kernel keeps its occupancy.
+struct FilterQuery {
+  const uint4* recs; const GeomDesc* descs; const RTCB200DeviceGeometry* geoms;
+  Ray r;                                  // the caller's world-space ray
+  RTCFilterFunctionN filter; RTCRayQueryContext* fctx; uint32_t instID, instPrimID; bool enforce;
+  float tfar;                             // out: the distance an accepting call left in ray.tfar
+  RTCHit best;                            // out: the hit of the last accepted candidate (closest hit)
+};
+
+// runIntersectionFilter1SYCL / runOcclusionFilter1SYCL (filter_sycl.h:83-108) for the candidate record ti at distance t; true =
+// accepted.  A candidate whose geometry does not enable the filter is accepted without a call.
 template <bool OCCLUDED, bool ROBUST, int GENERAL>
-__device__ __noinline__ void device_query1(const RTCB200DeviceTraversable t, RTCRay* ray, RTCHit* hitrec, uint32_t instID, uint32_t instPrimID) {
+__device__ __noinline__ bool offer_candidate(FilterQuery* q, uint32_t ti, float t, float u, float v, float cngx, float cngy, float cngz) {
+  const RTCB200DeviceGeometry& geom = q->geoms[__ldg(q->recs + (size_t)ti * 3 + 1).w];   // b.w: geomID or descriptor index
+  q->tfar = t;
+  if (!(q->enforce || geom.argFilterEnabled)) {   // the candidate is the hit: kept now, a later candidate overwrites u, v ...
+    if (!OCCLUDED) record_hit<ROBUST, GENERAL>(q->recs, q->descs, ti, q->r, u, v, cngx, cngy, cngz, q->instID, q->instPrimID, q->best);
+    return true;
+  }
+  RTCHit h;
+  record_hit<ROBUST, GENERAL>(q->recs, q->descs, ti, q->r, u, v, cngx, cngy, cngz, q->instID, q->instPrimID, h);
+  RTCRay fr;   // the caller's world-space ray, tfar = the candidate's t
+  fr.org_x = q->r.ox; fr.org_y = q->r.oy; fr.org_z = q->r.oz; fr.tnear = q->r.tnear;
+  fr.dir_x = q->r.dx; fr.dir_y = q->r.dy; fr.dir_z = q->r.dz; fr.time = q->r.time;
+  fr.tfar = t; fr.mask = q->r.mask; fr.id = q->r.id; fr.flags = q->r.flags;
+  RTCRayQueryContext fallback;
+  rtcInitRayQueryContext(&fallback);
+  RTCRayQueryContext* ctx = q->fctx ? q->fctx : &fallback;
+  const unsigned saveI = ctx->instID[0], saveP = ctx->instPrimID[0];
+  ctx->instID[0] = h.instID[0]; ctx->instPrimID[0] = h.instPrimID[0];   // instance_id_stack::push during an instanced traversal
+  int valid = -1;
+  RTCFilterFunctionNArguments fa;
+  fa.valid = &valid; fa.geometryUserPtr = geom.userPtr; fa.context = ctx;
+  fa.ray = reinterpret_cast<RTCRayN*>(&fr); fa.hit = reinterpret_cast<RTCHitN*>(&h); fa.N = 1;
+  q->filter(&fa);
+  ctx->instID[0] = saveI; ctx->instPrimID[0] = saveP;
+  if (valid == 0) return false;
+  if (!OCCLUDED) { q->best = h; q->tfar = fr.tfar; }   // copyHitToRay, and the distance the filter left
+  return true;
+}
+
+// FILTER: the arguments' filter `filter` runs on every candidate whose geometry enables it (`enforce`:
+// RTC_RAY_QUERY_FLAG_INVOKE_ARGUMENT_FILTER), as runIntersectionFilter1SYCL / runOcclusionFilter1SYCL do (filter_sycl.h:83-108);
+// geoms is the traversable's snapshot, fctx args->context.  Without FILTER the last four parameters are unused.
+template <bool OCCLUDED, bool ROBUST, int GENERAL, bool FILTER>
+__device__ __forceinline__ void query1(const RTCB200DeviceTraversable t, RTCRay* ray, RTCHit* hitrec, uint32_t instID, uint32_t instPrimID,
+                                       const RTCB200DeviceGeometry* geoms, RTCFilterFunctionN filter, RTCRayQueryContext* fctx, bool enforce) {
   const Node8* __restrict__ nodes = static_cast<const Node8*>(t.nodes);
   const uint4* __restrict__ recs = static_cast<const uint4*>(t.records);
   const GeomDesc* __restrict__ descs = static_cast<const GeomDesc*>(t.descs);
@@ -66,7 +186,7 @@ __device__ __noinline__ void device_query1(const RTCB200DeviceTraversable t, RTC
       if (GENERAL == 2 && d.kind != PRIM_TRIANGLE) {   // curve / point record: the winning test's normal is kept
         CurveHit ch;
         if (!(visible && curve_record_test(d, lr, tfar, a, b, c, ch))) return false;
-        if (!OCCLUDED) { tfar = ch.t; hit_u = ch.u; hit_v = ch.v; hit_rec = ti; cngx = ch.ngx; cngy = ch.ngy; cngz = ch.ngz; }
+        if (!OCCLUDED || FILTER) { tfar = ch.t; hit_u = ch.u; hit_v = ch.v; hit_rec = ti; cngx = ch.ngx; cngy = ch.ngy; cngz = ch.ngz; }
         return true;
       }
     }
@@ -76,7 +196,7 @@ __device__ __noinline__ void device_query1(const RTCB200DeviceTraversable t, RTC
       if (!tri_test_pluecker(lr, tfar, __uint_as_float(a.x), __uint_as_float(a.y), __uint_as_float(a.z), __uint_as_float(b.x),
                              __uint_as_float(b.y), __uint_as_float(b.z), __uint_as_float(c.x), __uint_as_float(c.y), __uint_as_float(c.z), ph))
         return false;
-      if (OCCLUDED) return true;
+      if (OCCLUDED && !FILTER) return true;   // an occlusion filter is handed the candidate's hit too
       tfar = ph.t; pluecker_uv(ph, hit_u, hit_v); hit_rec = ti;
       if (GENERAL && (a.w >> 31)) {   // second half of a quad (QuadHitPlueckerM::finalize, AVX form)
         const float u1 = sub_rn(1.0f, hit_u), v1 = sub_rn(1.0f, hit_v);
@@ -90,7 +210,7 @@ __device__ __noinline__ void device_query1(const RTCB200DeviceTraversable t, RTC
     if (!tri_test(lr, kSpread ? tfar0 : tfar, __uint_as_float(a.x), __uint_as_float(a.y), __uint_as_float(a.z), __uint_as_float(b.x),
                   __uint_as_float(b.y), __uint_as_float(b.z), __uint_as_float(c.x), __uint_as_float(c.y), __uint_as_float(c.z), th))
       return false;
-    if (OCCLUDED) return true;
+    if (OCCLUDED && !FILTER) return true;
     const float rcpAbsDen = 1.0f / th.absDen;   // finalize(): t,u,v = T,U,V * rcp(absDen)
     const float tt = th.T * rcpAbsDen;
     if (kSpread && !(tt <= tfar)) return false;
@@ -101,57 +221,91 @@ __device__ __noinline__ void device_query1(const RTCB200DeviceTraversable t, RTC
     hit_rec = ti;
     return true;
   };
+  // FILTER: a candidate the primitive test accepted is offered to the arguments' filter (offer_candidate); a rejected one leaves
+  // `tfar` as it was
+  FilterQuery q;
+  if (FILTER) {
+    q.recs = recs; q.descs = descs; q.geoms = geoms; q.r = r; q.filter = filter; q.fctx = fctx;
+    q.instID = instID; q.instPrimID = instPrimID; q.enforce = enforce;
+  }
+  auto ftest = [&](uint32_t ti, float& tfar) -> bool {
+    const float tprev = tfar;
+    if (!test(ti, tfar)) return false;
+    if (offer_candidate<OCCLUDED, ROBUST, GENERAL>(&q, ti, tfar, hit_u, hit_v, cngx, cngy, cngz)) { tfar = q.tfar; return true; }
+    tfar = tprev;
+    return false;
+  };
   const Ray r0 = r;   // the world-space ray: traverse_records shrinks r.tfar
-  if (!traverse_records<OCCLUDED, false>(r, rcp_safe_fast(r.dx), rcp_safe_fast(r.dy), rcp_safe_fast(r.dz), load_node, test, t.root_valid, nullptr))
-    return;
+  bool found;
+  if (FILTER) found = traverse_records<OCCLUDED, false>(r, rcp_safe_fast(r.dx), rcp_safe_fast(r.dy), rcp_safe_fast(r.dz), load_node, ftest, t.root_valid, nullptr);
+  else found = traverse_records<OCCLUDED, false>(r, rcp_safe_fast(r.dx), rcp_safe_fast(r.dy), rcp_safe_fast(r.dz), load_node, test, t.root_valid, nullptr);
+  if (!found) return;
   if (OCCLUDED) { ray->tfar = -INFINITY; return; }
-
-  // trace.cu write_back: Ng and the ids from the winning record; Ng stays in object space
-  const uint4* tp = recs + (size_t)hit_rec * 3;
-  const uint4 a = __ldg(tp), b = __ldg(tp + 1), c = __ldg(tp + 2);
-  float ngx, ngy, ngz;
-  uint32_t primID = a.w, geomID = b.w;
-  float lox = r0.ox, loy = r0.oy, loz = r0.oz;   // ray origin in the space the record's triangle lives in
-  bool curve_hit = false;
-  if (GENERAL) {
-    const GeomDesc& d = descs[b.w];
-    geomID = d.geomID;
-    if (GENERAL == 2 && d.kind != PRIM_TRIANGLE) { ngx = cngx; ngy = cngy; ngz = cngz; curve_hit = true; }
-    if (d.has_xfm) {
-      instID = d.instID; instPrimID = 0u;   // instance_id_stack::push(context, instID, 0)
-      if (ROBUST) { Ray lr = r0; to_object_space(d, lr); lox = lr.ox; loy = lr.oy; loz = lr.oz; }
-    }
+  if (FILTER) {
+    ray->tfar = r.tfar;
+    const RTCHit& b = q.best;
+    hitrec->Ng_x = b.Ng_x; hitrec->Ng_y = b.Ng_y; hitrec->Ng_z = b.Ng_z; hitrec->u = b.u; hitrec->v = b.v;
+    hitrec->primID = b.primID; hitrec->geomID = b.geomID; hitrec->instID[0] = b.instID[0]; hitrec->instPrimID[0] = b.instPrimID[0];
+    return;
   }
-  if (curve_hit) {
-  } else if (ROBUST) {   // stable_triangle_normal of the origin-relative edges, exactly as in tri_test_pluecker
-    const float v0x = sub_rn(__uint_as_float(a.x), lox), v0y = sub_rn(__uint_as_float(a.y), loy), v0z = sub_rn(__uint_as_float(a.z), loz);
-    const float v1x = sub_rn(__uint_as_float(b.x), lox), v1y = sub_rn(__uint_as_float(b.y), loy), v1z = sub_rn(__uint_as_float(b.z), loz);
-    const float v2x = sub_rn(__uint_as_float(c.x), lox), v2y = sub_rn(__uint_as_float(c.y), loy), v2z = sub_rn(__uint_as_float(c.z), loz);
-    stable_normal(sub_rn(v2x, v0x), sub_rn(v2y, v0y), sub_rn(v2z, v0z), sub_rn(v0x, v1x), sub_rn(v0y, v1y), sub_rn(v0z, v1z),
-                  sub_rn(v1x, v2x), sub_rn(v1y, v2y), sub_rn(v1z, v2z), ngx, ngy, ngz);
-  } else {
-    const float e1x = __uint_as_float(b.x), e1y = __uint_as_float(b.y), e1z = __uint_as_float(b.z);
-    const float e2x = __uint_as_float(c.x), e2y = __uint_as_float(c.y), e2z = __uint_as_float(c.z);
-    ngx = msub(e2y, e1z, mul_rn(e2z, e1y));
-    ngy = msub(e2z, e1x, mul_rn(e2x, e1z));
-    ngz = msub(e2x, e1y, mul_rn(e2y, e1x));
-  }
-  if (GENERAL && !curve_hit && (a.w >> 31)) {   // quad halves share the quad's primID; the second one has flipped winding
-    primID = a.w & 0x7FFFFFFFu;
-    ngx = -ngx; ngy = -ngy; ngz = -ngz;
-  }
+  RTCHit h;
+  record_hit<ROBUST, GENERAL>(recs, descs, hit_rec, r0, hit_u, hit_v, cngx, cngy, cngz, instID, instPrimID, h);
   ray->tfar = r.tfar;
-  hitrec->Ng_x = ngx; hitrec->Ng_y = ngy; hitrec->Ng_z = ngz; hitrec->u = hit_u; hitrec->v = hit_v;
-  hitrec->primID = primID; hitrec->geomID = geomID; hitrec->instID[0] = instID; hitrec->instPrimID[0] = instPrimID;
+  hitrec->Ng_x = h.Ng_x; hitrec->Ng_y = h.Ng_y; hitrec->Ng_z = h.Ng_z; hitrec->u = h.u; hitrec->v = h.v;
+  hitrec->primID = h.primID; hitrec->geomID = h.geomID; hitrec->instID[0] = h.instID[0]; hitrec->instPrimID[0] = h.instPrimID[0];
 }
 
-// the specialisation the batched kernel would run for this scene (trace.cu launch_k)
+// One query of one thread, as its own function: the six variants without a filter and the six with one.
+template <bool OCCLUDED, bool ROBUST, int GENERAL>
+__device__ __noinline__ void device_query1(const RTCB200DeviceTraversable t, RTCRay* ray, RTCHit* hitrec, uint32_t instID, uint32_t instPrimID) {
+  query1<OCCLUDED, ROBUST, GENERAL, false>(t, ray, hitrec, instID, instPrimID, nullptr, nullptr, nullptr, false);
+}
+template <bool OCCLUDED, bool ROBUST, int GENERAL>
+__device__ __noinline__ void device_query1_filter(const RTCB200DeviceTraversable t, RTCRay* ray, RTCHit* hitrec, uint32_t instID, uint32_t instPrimID,
+                                                  RTCFilterFunctionN filter, RTCRayQueryContext* fctx, bool enforce) {
+  query1<OCCLUDED, ROBUST, GENERAL, true>(t, ray, hitrec, instID, instPrimID, t.geometries, filter, fctx, enforce);
+}
+
+// The filtered specialisations, compiled only into kernels that ask for argument filters (FILTERS): run when the arguments carry a
+// filter and their feature_mask admits it (filter_sycl.h:32-43); false when the query is left to the unfiltered ones.
+template <bool OCCLUDED, bool FILTERS>
+struct FilterDispatch {
+  template <typename Args>
+  static __device__ __forceinline__ bool run(const RTCB200DeviceTraversable&, RTCRay*, RTCHit*, const Args*, uint32_t, uint32_t, int) { return false; }
+};
 template <bool OCCLUDED>
-__device__ __forceinline__ void device_query1_dispatch(const RTCB200DeviceTraversable& t, RTCRay* ray, RTCHit* hit, const RTCRayQueryContext* ctx) {
+struct FilterDispatch<OCCLUDED, true> {
+  template <typename Args>
+  static __device__ __forceinline__ bool run(const RTCB200DeviceTraversable& t, RTCRay* ray, RTCHit* hit, const Args* args, uint32_t instID,
+                                             uint32_t instPrimID, int variant) {
+    if (!(args && args->filter && (args->feature_mask & RTC_FEATURE_FLAG_FILTER_FUNCTION_IN_ARGUMENTS))) return false;
+    const RTCFilterFunctionN f = args->filter;
+    RTCRayQueryContext* fctx = args->context;
+    const bool enforce = (args->flags & RTC_RAY_QUERY_FLAG_INVOKE_ARGUMENT_FILTER) != 0;
+    switch (variant) {
+      case 0: device_query1_filter<OCCLUDED, false, 0>(t, ray, hit, instID, instPrimID, f, fctx, enforce); break;
+      case 1: device_query1_filter<OCCLUDED, true, 0>(t, ray, hit, instID, instPrimID, f, fctx, enforce); break;
+      case 2: device_query1_filter<OCCLUDED, false, 1>(t, ray, hit, instID, instPrimID, f, fctx, enforce); break;
+      case 3: device_query1_filter<OCCLUDED, true, 1>(t, ray, hit, instID, instPrimID, f, fctx, enforce); break;
+      case 4: device_query1_filter<OCCLUDED, false, 2>(t, ray, hit, instID, instPrimID, f, fctx, enforce); break;
+      default: device_query1_filter<OCCLUDED, true, 2>(t, ray, hit, instID, instPrimID, f, fctx, enforce); break;
+    }
+    return true;
+  }
+};
+
+// the specialisation the batched kernel would run for this scene (trace.cu launch_k); with FEATURES containing
+// RTC_FEATURE_FLAG_FILTER_FUNCTION_IN_ARGUMENTS, the filtered one when the arguments carry a filter
+template <bool OCCLUDED, unsigned FEATURES, typename Args>
+__device__ __forceinline__ void device_query1_dispatch(const RTCB200DeviceTraversable& t, RTCRay* ray, RTCHit* hit, const Args* args) {
+  const RTCRayQueryContext* ctx = args ? args->context : nullptr;
   if (!t.root_valid) return;   // empty scene
   uint32_t instID = RTC_INVALID_GEOMETRY_ID, instPrimID = RTC_INVALID_GEOMETRY_ID;
   if (ctx) { instID = ctx->instID[0]; instPrimID = ctx->instPrimID[0]; }
   const int g = !t.descs ? 0 : (t.curves ? 2 : 1);
+  if (FilterDispatch<OCCLUDED, (FEATURES & RTC_FEATURE_FLAG_FILTER_FUNCTION_IN_ARGUMENTS) != 0>::run(t, ray, hit, args, instID, instPrimID,
+                                                                                                    g * 2 + (t.robust ? 1 : 0)))
+    return;
   switch (g * 2 + (t.robust ? 1 : 0)) {
     case 0: device_query1<OCCLUDED, false, 0>(t, ray, hit, instID, instPrimID); break;
     case 1: device_query1<OCCLUDED, true, 0>(t, ray, hit, instID, instPrimID); break;
@@ -164,13 +318,24 @@ __device__ __forceinline__ void device_query1_dispatch(const RTCB200DeviceTraver
 
 }  // namespace rtk
 
-// Closest hit of one ray: as one record of rtcb200Intersect1MDevice.
+// Closest hit of one ray: as one record of rtcb200Intersect1MDevice.  No filter code is compiled in: args->filter is not called.
 __device__ __forceinline__ void rtcb200TraversableIntersect1(const RTCB200DeviceTraversable& t, RTCRayHit* rayhit,
                                                              const RTCIntersectArguments* args = nullptr) {
-  rtk::device_query1_dispatch<false>(t, &rayhit->ray, &rayhit->hit, args ? args->context : nullptr);
+  rtk::device_query1_dispatch<false, RTC_FEATURE_FLAG_NONE>(t, &rayhit->ray, &rayhit->hit, args);
 }
-// Any hit of one ray: as one record of rtcb200Occluded1MDevice (tfar = -inf on a hit).
+// Any hit of one ray: as one record of rtcb200Occluded1MDevice (tfar = -inf on a hit).  No filter code is compiled in.
 __device__ __forceinline__ void rtcb200TraversableOccluded1(const RTCB200DeviceTraversable& t, RTCRay* ray,
                                                             const RTCOccludedArguments* args = nullptr) {
-  rtk::device_query1_dispatch<true>(t, ray, nullptr, args ? args->context : nullptr);
+  rtk::device_query1_dispatch<true, RTC_FEATURE_FLAG_NONE>(t, ray, nullptr, args);
+}
+// The same with the features the kernel is compiled for (Embree 4's SYCL feature-mask specialisation):
+// rtcb200TraversableIntersect1<RTC_FEATURE_FLAG_FILTER_FUNCTION_IN_ARGUMENTS>(t, &rh, &args) compiles the filtered variants into
+// the kernel and runs them when args->filter is set and args->feature_mask admits it.  Other feature bits change nothing.
+template <unsigned FEATURES>
+__device__ __forceinline__ void rtcb200TraversableIntersect1(const RTCB200DeviceTraversable& t, RTCRayHit* rayhit, const RTCIntersectArguments* args) {
+  rtk::device_query1_dispatch<false, FEATURES>(t, &rayhit->ray, &rayhit->hit, args);
+}
+template <unsigned FEATURES>
+__device__ __forceinline__ void rtcb200TraversableOccluded1(const RTCB200DeviceTraversable& t, RTCRay* ray, const RTCOccludedArguments* args) {
+  rtk::device_query1_dispatch<true, FEATURES>(t, ray, nullptr, args);
 }
