@@ -16,7 +16,7 @@
 
 namespace rtk {
 
-// what a geometry interpolates as (the kind of an interpolation table entry, rtk_device.h InterpEntry)
+// what a geometry interpolates as (the kind of an interpolation table entry, InterpEntry below)
 enum InterpKind : uint32_t {
   INTERP_NONE = 0,            // nothing to interpolate (points, missing buffer or slot): quiet NaN
   INTERP_TRIANGLE = 1,
@@ -29,6 +29,21 @@ enum InterpKind : uint32_t {
 };
 RT_HD constexpr bool interp_curve(uint32_t kind) { return kind >= INTERP_LINEAR && kind <= INTERP_HERMITE_ATTRIB; }
 RT_HD constexpr int interp_index_count(uint32_t kind) { return kind == INTERP_TRIANGLE ? 3 : kind == INTERP_QUAD ? 4 : 1; }
+
+// One entry of a scene's device interpolation table (rtcb200InterpolateHits*, rtcb200GetSceneDeviceInterpolator): one entry per
+// geomID of the scene, then one block of entries per instanced scene: an INTERP_INSTANCE entry's `sub` is the first entry of its
+// scene's block and `nprims` the block's length, so a hit resolves in at most two lookups.  Buffers are device copies (stride honoured).
+struct InterpEntry {
+  uint32_t kind = 0;             // InterpKind
+  uint32_t basis = 0;            // INTERP_CUBIC: CurveBasis
+  uint32_t nprims = 0;           // primitives (INTERP_INSTANCE: entries of the sub-table)
+  uint32_t sub = 0;              // INTERP_INSTANCE: first entry of the sub-table
+  const uint8_t* idx = nullptr;  // index buffer
+  const uint8_t* data = nullptr; // the requested vertex / attribute buffer
+  const uint8_t* tang = nullptr; // INTERP_HERMITE: the tangent buffer
+  uint64_t istride = 0, dstride = 0, tstride = 0;
+  uint64_t nelems = 0, ntang = 0;   // elements of the data / tangent buffer: an index beyond them gives NaN, not a wild read
+};
 
 // One primitive at (u, v): the buffer elements its control values come from and the weights they are combined with.
 // row[0..3]: element indices into the requested buffer, except for INTERP_HERMITE, whose row[2], row[3] index the tangent
@@ -164,5 +179,78 @@ RT_HD void interpolate_prim(uint32_t kind, uint32_t basis, const uint32_t* idx, 
       if (out[c]) out[c][(uint64_t)k * ostride] = o[c];
   }
 }
+
+#if defined(__CUDACC__)
+// One hit of the device interpolation: the batched kernel (interpolate.cu) and rtcb200Interpolate1 (include/embree4_b200_device.cuh)
+// both run this body; only where value k goes differs, so `store(k, o)` writes the six outputs o (P, dPdu, dPdv, ddPdudu, ddPdvdv,
+// ddPdudv) of value k.  The hit is geometry geomID of the table's scene, or, with instID valid, geometry geomID of the scene
+// instance instID instantiates.  Points, instances, a missing buffer or slot and an index beyond a buffer store quiet NaN.
+template <typename Store>
+__device__ __forceinline__ void interpolate_hit(const InterpEntry* table,uint32_t nentries, uint32_t geomID, uint32_t instID,
+                                                uint32_t primID, float u, float v, unsigned V, Store store) {
+  // resolve the entry: the scene's own geometry, or geometry geomID of the scene instance instID instantiates
+  InterpEntry e;
+  e.kind = INTERP_NONE;
+  uint32_t slot = geomID, end = nentries;
+  bool ok = true;
+  if (instID != kInvalidID) {
+    ok = instID < nentries && table[instID].kind == INTERP_INSTANCE;
+    if (ok) { slot = table[instID].sub + geomID; end = table[instID].sub + table[instID].nprims; ok = geomID < table[instID].nprims; }
+  }
+  if (ok && slot < end) e = table[slot];
+  const uint32_t kind = e.kind;
+  InterpPrim s;
+  bool valid = kind != INTERP_NONE && kind != INTERP_INSTANCE && primID < e.nprims;
+  if (valid) {
+    uint32_t idx[4] = {0, 0, 0, 0};
+    const uint32_t* ip = reinterpret_cast<const uint32_t*>(e.idx + (uint64_t)primID * e.istride);
+    const int ni = interp_index_count(kind);
+#pragma unroll
+    for (int k = 0; k < 4; ++k)
+      if (k < ni) idx[k] = __ldg(ip + k);
+    s = interp_prim(kind, e.basis, idx, u, v);
+    // every element read must lie in its buffer
+#pragma unroll
+    for (int r = 0; r < 4; ++r)
+      if (r < s.nrows) valid = valid && (uint64_t)s.row[r] < ((kind == INTERP_HERMITE && r >= 2) ? e.ntang : e.nelems);
+  }
+  if (!valid) {
+    const float o[6] = {__int_as_float(0x7FC00000), __int_as_float(0x7FC00000), __int_as_float(0x7FC00000),
+                        __int_as_float(0x7FC00000), __int_as_float(0x7FC00000), __int_as_float(0x7FC00000)};
+    for (unsigned k = 0; k < V; ++k) store(k, o);
+    return;
+  }
+  const uint8_t* rows[4];
+#pragma unroll
+  for (int r = 0; r < 4; ++r)
+    rows[r] = (kind == INTERP_HERMITE && r >= 2) ? e.tang + (uint64_t)s.row[r] * e.tstride : e.data + (uint64_t)s.row[r] * e.dstride;
+  unsigned k = 0;
+  // 16-byte loads where every row is 16-byte aligned
+  const bool vec = ((reinterpret_cast<uintptr_t>(e.data) | e.dstride) & 15) == 0 &&
+                   (kind != INTERP_HERMITE || ((reinterpret_cast<uintptr_t>(e.tang) | e.tstride) & 15) == 0);
+  if (vec) {
+    for (; k + 4 <= V; k += 4) {
+      float4 q[4];
+#pragma unroll
+      for (int r = 0; r < 4; ++r) q[r] = r < s.nrows ? __ldg(reinterpret_cast<const float4*>(rows[r] + 4ull * k)) : make_float4(0.f, 0.f, 0.f, 0.f);
+      const float c0[4] = {q[0].x, q[1].x, q[2].x, q[3].x}, c1[4] = {q[0].y, q[1].y, q[2].y, q[3].y};
+      const float c2[4] = {q[0].z, q[1].z, q[2].z, q[3].z}, c3[4] = {q[0].w, q[1].w, q[2].w, q[3].w};
+      float o[6];
+      interp_value(kind, s, c0, o); store(k, o);
+      interp_value(kind, s, c1, o); store(k + 1, o);
+      interp_value(kind, s, c2, o); store(k + 2, o);
+      interp_value(kind, s, c3, o); store(k + 3, o);
+    }
+  }
+  for (; k < V; ++k) {
+    float c[4] = {0.f, 0.f, 0.f, 0.f}, o[6];
+#pragma unroll
+    for (int r = 0; r < 4; ++r)
+      if (r < s.nrows) c[r] = __ldg(reinterpret_cast<const float*>(rows[r]) + k);
+    interp_value(kind, s, c, o);
+    store(k, o);
+  }
+}
+#endif
 
 }  // namespace rtk

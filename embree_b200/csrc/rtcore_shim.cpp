@@ -25,6 +25,7 @@
 #include "../../include/embree4_b200.h"
 #include "interp.cuh"
 #include "rtk_device.h"
+#include "transform_format.cuh"
 
 namespace {
 
@@ -229,12 +230,13 @@ struct SceneImpl : RefCounted {
   // copies of the buffers it reads; built by the first call that needs it, freed by the next commit and with the scene
   struct InterpTable { RTCBufferType type; unsigned slot; rtk::InterpEntry* d_table; uint32_t nentries; std::vector<void*> buffers; };
   std::vector<InterpTable> interpTables;
-  // device-side argument filters (rtcb200GetSceneDeviceTraversable): (geomID, instID or invalid) of every descriptor of the last
-  // commit, and the {userPtr, argFilterEnabled} snapshots the getter uploaded since then -- the newest is reused while it is
+  // device-side argument filters and shading getters (rtcb200GetSceneDeviceTraversable): (geomID, instID or invalid) of every
+  // descriptor of the last commit, and the geometry snapshots the getter uploaded since then (geometry_snapshot: header,
+  // per-record table, per-geomID block in one allocation) with the bytes of the newest after its header -- reused while they are
   // unchanged; the next commit frees them all, and so does releasing the scene
   std::vector<std::pair<uint32_t, uint32_t>> descIds;
   std::vector<void*> geomTables;
-  std::vector<RTCB200DeviceGeometry> lastGeomTable;
+  std::vector<unsigned char> lastGeomTable;
   void free_geom_tables() {
     for (void* p : geomTables) cudaFreeAsync(p, 0);
     geomTables.clear(); lastGeomTable.clear();
@@ -1385,21 +1387,25 @@ static bool check_interpolate_hits(SceneImpl* s, const RTCB200InterpolateHitsArg
   return a->M && a->valueCount && (a->P || a->dPdu || a->ddPdudu);
 }
 
+// the scene's interpolation table for (type, slot), built on `st` by the first request since the last commit -- of the batched calls
+// or of rtcb200GetSceneDeviceInterpolator, which share it; complete on the device when this returns
+static SceneImpl::InterpTable* interp_table(SceneImpl* s, RTCBufferType type, unsigned slot, cudaStream_t st) {
+  for (SceneImpl::InterpTable& x : s->interpTables) if (x.type == type && x.slot == slot) return &x;
+  s->interpTables.push_back(SceneImpl::InterpTable{type, slot, nullptr, 0, {}});
+  SceneImpl::InterpTable* t = &s->interpTables.back();
+  try { InterpTableBuild{s, *t, st, {}}.build(); }
+  catch (...) {   // a partly built table is not kept
+    if (t->d_table) cudaFreeAsync(t->d_table, st);
+    for (void* p : t->buffers) cudaFreeAsync(p, st);
+    s->interpTables.pop_back();
+    throw;
+  }
+  return t;
+}
+
 // enqueues the interpolation of `a` (hits and outputs in device memory) on `st`
 static void interpolate_hits(SceneImpl* s, const RTCB200InterpolateHitsArguments* a, const RTCRayHit* d_hits, float* const d_out[6], cudaStream_t st) {
-  SceneImpl::InterpTable* t = nullptr;
-  for (SceneImpl::InterpTable& x : s->interpTables) if (x.type == a->bufferType && x.slot == a->bufferSlot) t = &x;
-  if (!t) {
-    s->interpTables.push_back(SceneImpl::InterpTable{a->bufferType, a->bufferSlot, nullptr, 0, {}});
-    t = &s->interpTables.back();
-    try { InterpTableBuild{s, *t, st, {}}.build(); }
-    catch (...) {   // a partly built table is not kept
-      if (t->d_table) cudaFreeAsync(t->d_table, st);
-      for (void* p : t->buffers) cudaFreeAsync(p, st);
-      s->interpTables.pop_back();
-      throw;
-    }
-  }
+  const SceneImpl::InterpTable* t = interp_table(s, a->bufferType, a->bufferSlot, st);
   rtk::InterpParams p;
   p.hits = d_hits; p.M = a->M; p.table = t->d_table; p.nentries = t->nentries; p.valueCount = a->valueCount;
   for (int c = 0; c < 6; ++c) p.out[c] = d_out[c];
@@ -1741,12 +1747,17 @@ void rtcb200GetSceneStats(RTCScene sc, struct RTCB200SceneStats* o) {
   }
   SCENE_END
 }
-// What the device-side argument filters read about the geometry of a record (embree4_b200.h RTCB200DeviceGeometry), one entry per
-// value of a record's b.w: the geomID in a triangle-only scene, the descriptor index otherwise, an instanced descriptor taking its
-// child geometry's values -- the geometry hit_geometry() finds for the host-pointer path.  User data and the filter switch change
-// without a commit, so every call takes them anew; an unchanged table is not uploaded twice.  Called with commitMutex held.
+// What device code reads about a scene's geometries, in one allocation (embree4_b200.h RTCB200DeviceGeometryHeader):
+//  - the header: where the geomID block is and how many ids it covers;
+//  - what the argument filters read about the geometry of a record (RTCB200DeviceGeometry), one entry per value of a record's b.w:
+//    the geomID in a triangle-only scene, the descriptor index otherwise, an instanced descriptor taking its child geometry's
+//    values -- the geometry hit_geometry() finds for the host-pointer path.  The returned pointer is its first entry;
+//  - the geomID block the shading getters read (RTCB200DeviceGeometryInfo): user data, and an instance's local-to-world transform.
+// User data, the filter switch and transforms change without a commit, so every call takes them anew; unchanged contents are not
+// uploaded twice.  Called with commitMutex held.
 static const RTCB200DeviceGeometry* geometry_snapshot(SceneImpl* s) {
   std::vector<RTCB200DeviceGeometry> tab;
+  std::vector<RTCB200DeviceGeometryInfo> ids;
   auto entry = [](const GeometryImpl* g) {
     RTCB200DeviceGeometry e;
     memset(&e, 0, sizeof e);
@@ -1755,6 +1766,16 @@ static const RTCB200DeviceGeometry* geometry_snapshot(SceneImpl* s) {
   };
   {
     std::lock_guard<std::mutex> lg(s->geomMutex);
+    for (const GeometryImpl* g : s->geoms) {
+      RTCB200DeviceGeometryInfo e;
+      memset(&e, 0, sizeof e);
+      if (g) {
+        e.userPtr = g->userPtr;
+        e.isInstance = g->type == RTC_GEOMETRY_TYPE_INSTANCE ? 1u : 0u;
+        if (e.isInstance) memcpy(e.xfm, g->xfm, sizeof e.xfm);
+      }
+      ids.push_back(e);
+    }
     if (!s->gpu.general) {
       for (const GeometryImpl* g : s->geoms) tab.push_back(entry(g));
     } else {
@@ -1771,20 +1792,31 @@ static const RTCB200DeviceGeometry* geometry_snapshot(SceneImpl* s) {
     }
   }
   if (tab.empty()) tab.push_back(entry(nullptr));
-  const size_t bytes = tab.size() * sizeof(RTCB200DeviceGeometry);
-  if (!s->geomTables.empty() && tab.size() == s->lastGeomTable.size() && memcmp(tab.data(), s->lastGeomTable.data(), bytes) == 0)
-    return static_cast<const RTCB200DeviceGeometry*>(s->geomTables.back());
+  static_assert(sizeof(RTCB200DeviceGeometryHeader) == sizeof(RTCB200DeviceGeometry), "the header takes the place of one entry");
+  const size_t head = sizeof(RTCB200DeviceGeometryHeader), tabBytes = tab.size() * sizeof(RTCB200DeviceGeometry);
+  std::vector<unsigned char> blob(head + tabBytes + ids.size() * sizeof(RTCB200DeviceGeometryInfo));
+  memcpy(blob.data() + head, tab.data(), tabBytes);
+  if (!ids.empty()) memcpy(blob.data() + head + tabBytes, ids.data(), ids.size() * sizeof(RTCB200DeviceGeometryInfo));
+  // the header holds the allocation's own address: the contents after it decide whether the last snapshot still holds
+  if (!s->geomTables.empty() && blob.size() == s->lastGeomTable.size() &&
+      memcmp(blob.data() + head, s->lastGeomTable.data() + head, blob.size() - head) == 0)
+    return reinterpret_cast<const RTCB200DeviceGeometry*>(static_cast<const char*>(s->geomTables.back()) + head);
   // on the calling thread's own non-blocking stream: the upload waits for no other work, and is complete when the getter returns
   // (the caller's kernels run on streams of their own)
   s->dev->use();
   t_ctx.ensure(s->dev->gpu);
   void* p = nullptr;
-  cuda_check(cudaMallocAsync(&p, bytes, t_ctx.stream), "cudaMallocAsync(geometry table)");
+  cuda_check(cudaMallocAsync(&p, blob.size(), t_ctx.stream), "cudaMallocAsync(geometry table)");
   s->geomTables.push_back(p);
-  cuda_check(cudaMemcpyAsync(p, tab.data(), bytes, cudaMemcpyHostToDevice, t_ctx.stream), "upload geometry table");
+  RTCB200DeviceGeometryHeader h;
+  memset(&h, 0, sizeof h);
+  h.byGeomID = ids.empty() ? nullptr : reinterpret_cast<const RTCB200DeviceGeometryInfo*>(static_cast<const char*>(p) + head + tabBytes);
+  h.count = (unsigned)ids.size();
+  memcpy(blob.data(), &h, head);
+  cuda_check(cudaMemcpyAsync(p, blob.data(), blob.size(), cudaMemcpyHostToDevice, t_ctx.stream), "upload geometry table");
   cuda_check(cudaStreamSynchronize(t_ctx.stream), "upload geometry table");
-  s->lastGeomTable.swap(tab);
-  return static_cast<const RTCB200DeviceGeometry*>(p);
+  s->lastGeomTable.swap(blob);
+  return reinterpret_cast<const RTCB200DeviceGeometry*>(static_cast<const char*>(p) + head);
 }
 
 // the arrays trace_device hands the kernel (make_params), for device-side queries; refused where trace_device would refuse
@@ -1799,12 +1831,31 @@ void rtcb200GetSceneDeviceTraversable(RTCScene sc, struct RTCB200DeviceTraversab
   if (filters_apply(s, none, 0) || filters_apply(s, none, 1))
     fail(RTC_ERROR_INVALID_OPERATION, "filter callbacks are host functions: device-side queries cannot call them");
   const rtk::SceneGPU& g = s->gpu;
-  const RTCB200DeviceGeometry* geoms = g.root_valid ? geometry_snapshot(s) : nullptr;
+  bool any;   // a scene without primitives still answers its geometries' user data
+  { std::lock_guard<std::mutex> lg(s->geomMutex); any = !s->geoms.empty(); }
+  const RTCB200DeviceGeometry* geoms = any ? geometry_snapshot(s) : nullptr;
   o->nodes = g.nodes; o->records = g.tris;
   o->descs = g.general ? g.d_descs : nullptr;
   o->root_valid = g.root_valid; o->robust = (unsigned)g.robust; o->general = (unsigned short)g.general; o->curves = (unsigned)g.curves;
   o->device = (short)s->dev->gpu;
   o->geometries = geoms;
+  SCENE_END
+}
+// the interpolation table the batched calls use for (type, slot), for rtcb200Interpolate1 in the caller's kernels; refused where the
+// batched calls refuse the scene or the buffer
+void rtcb200GetSceneDeviceInterpolator(RTCScene sc, enum RTCBufferType type, unsigned int slot, struct RTCB200DeviceInterpolator* o) {
+  SCENE_BEGIN(sc)
+  VERIFY_HANDLE(o);
+  memset(o, 0, sizeof *o);
+  SceneImpl* s = S(sc);
+  std::lock_guard<std::mutex> lk(s->commitMutex);
+  { std::lock_guard<std::mutex> lg(s->geomMutex); if (!s->everCommitted || s->isModified()) fail(RTC_ERROR_INVALID_OPERATION, "scene not committed"); }
+  if (type == RTC_BUFFER_TYPE_VERTEX ? slot != 0 : type != RTC_BUFFER_TYPE_VERTEX_ATTRIBUTE) fail(RTC_ERROR_INVALID_OPERATION, "invalid buffer");
+  // built on the calling thread's own stream, like the geometry snapshot: the caller's kernels run on streams of their own
+  s->dev->use();
+  t_ctx.ensure(s->dev->gpu);
+  const SceneImpl::InterpTable* t = interp_table(s, type, slot, t_ctx.stream);
+  o->table = t->d_table; o->nentries = t->nentries;
   SCENE_END
 }
 static void scene_layout(const rtk::SceneGPU& g, RTCB200SceneLayout* o) {
@@ -1940,13 +1991,8 @@ static void load_transform(RTCFormat format, const float* x, float out[12]) {   
     default: fail(RTC_ERROR_INVALID_OPERATION, "invalid matrix format");
   }
 }
-static void store_transform(const float m[12], RTCFormat format, float* x) {    // storeTransform, rtcore.cpp
-  switch ((int)format) {
-    case 0x9134: { const float o[12] = {m[0], m[3], m[6], m[9], m[1], m[4], m[7], m[10], m[2], m[5], m[8], m[11]}; memcpy(x, o, sizeof o); break; }
-    case 0x9234: memcpy(x, m, 12 * sizeof(float)); break;
-    case 0x9244: { const float o[16] = {m[0], m[1], m[2], 0, m[3], m[4], m[5], 0, m[6], m[7], m[8], 0, m[9], m[10], m[11], 1}; memcpy(x, o, sizeof o); break; }
-    default: fail(RTC_ERROR_INVALID_OPERATION, "invalid matrix format");
-  }
+static void store_transform(const float m[12], RTCFormat format, float* x) {    // storeTransform: transform_format.cuh, shared with the device
+  if (!rtk::store_transform(m, (unsigned)format, x)) fail(RTC_ERROR_INVALID_OPERATION, "invalid matrix format");
 }
 void rtcSetGeometryInstancedScene(RTCGeometry g, RTCScene scene) {
   GEOM_BEGIN(g)

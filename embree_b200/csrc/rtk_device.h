@@ -157,20 +157,8 @@ struct TraceParams {
 // occluded: 0 = closest hit (rtcIntersect*), 1 = any hit (rtcOccluded*); K in {1,4,8,16}
 int launch_trace(const TraceParams& p, int occluded, int K, cudaStream_t stream);
 
-// ---- batched interpolation of hits (interpolate.cu; interp.cuh holds the arithmetic).  One entry per geomID of a scene, then one
-// block of entries per instanced scene: an INTERP_INSTANCE entry's `sub` is the first entry of its scene's block and `nprims` the
-// block's length, so a hit resolves in at most two lookups.  Buffers are device copies (stride honoured).
-struct InterpEntry {
-  uint32_t kind = 0;             // InterpKind
-  uint32_t basis = 0;            // INTERP_CUBIC: CurveBasis
-  uint32_t nprims = 0;           // primitives (INTERP_INSTANCE: entries of the sub-table)
-  uint32_t sub = 0;              // INTERP_INSTANCE: first entry of the sub-table
-  const uint8_t* idx = nullptr;  // index buffer
-  const uint8_t* data = nullptr; // the requested vertex / attribute buffer
-  const uint8_t* tang = nullptr; // INTERP_HERMITE: the tangent buffer
-  uint64_t istride = 0, dstride = 0, tstride = 0;
-  uint64_t nelems = 0, ntang = 0;   // elements of the data / tangent buffer: an index beyond them gives NaN, not a wild read
-};
+// ---- batched interpolation of hits (interpolate.cu; interp.cuh holds the table entry, the per-hit code and the arithmetic)
+struct InterpEntry;
 struct InterpParams {
   const void* hits;              // RTCRayHit[M]
   unsigned long long M;

@@ -226,6 +226,29 @@ class DeviceGeometry(C.Structure):
     _fields_ = [("userPtr", C.c_void_p), ("argFilterEnabled", C.c_uint)]
 
 
+class DeviceGeometryInfo(C.Structure):
+    """RTCB200DeviceGeometryInfo: one entry of the snapshot's geomID block, what the device-side shading getters read."""
+    _fields_ = [("userPtr", C.c_void_p), ("isInstance", C.c_uint), ("xfm", C.c_float * 12)]
+
+
+class DeviceGeometryHeader(C.Structure):
+    """RTCB200DeviceGeometryHeader: the 16 bytes in front of DeviceTraversable.geometries[0]."""
+    _fields_ = [("byGeomID", C.c_void_p), ("count", C.c_uint), ("reserved", C.c_uint)]
+
+
+class DeviceInterpolator(C.Structure):
+    """RTCB200DeviceInterpolator (include/embree4_b200.h, Section B): a scene's interpolation table for one buffer, passed to kernels
+    that call rtcb200Interpolate1 (include/embree4_b200_device.cuh)."""
+    _fields_ = [("table", C.c_void_p), ("nentries", C.c_uint), ("reserved", C.c_uint)]
+
+
+class DeviceInterpolateArguments(C.Structure):
+    """RTCB200DeviceInterpolateArguments: rtcb200Interpolate1's arguments (device memory or the calling thread's own)."""
+    _fields_ = [("geomID", C.c_uint), ("instID", C.c_uint), ("primID", C.c_uint), ("u", C.c_float), ("v", C.c_float),
+                ("P", C.c_void_p), ("dPdu", C.c_void_p), ("dPdv", C.c_void_p), ("ddPdudu", C.c_void_p), ("ddPdvdv", C.c_void_p),
+                ("ddPdudv", C.c_void_p), ("valueCount", C.c_uint)]
+
+
 DESC_DTYPE = np.dtype([("geomID", "<u4"), ("instID", "<u4"), ("kind", "<u4"), ("first", "<u4"), ("count", "<u4"), ("is_quad", "<u4"),
                        ("tess", "<u4"), ("basis", "<u4"), ("hermite", "<u4"), ("xfm", "<f4", (12,))])   # RTCB200DescInfo
 
@@ -327,6 +350,7 @@ class RTCLib:
         "rtcb200InterpolateHits": (None, [C.c_void_p, C.c_void_p]),
         "rtcb200InterpolateHitsDevice": (None, [C.c_void_p, C.c_void_p, C.c_void_p]),
         "rtcb200GetSceneDeviceTraversable": (None, [C.c_void_p, C.c_void_p]),
+        "rtcb200GetSceneDeviceInterpolator": (None, [C.c_void_p, C.c_int, C.c_uint, C.c_void_p]),
     }
 
     def __init__(self, path):
@@ -565,6 +589,13 @@ class RTCLib:
         t = DeviceTraversable()
         self.rtcb200GetSceneDeviceTraversable(scene, C.byref(t))
         return t
+
+    def scene_device_interpolator(self, scene, buffer_type, slot=0):
+        """rtcb200GetSceneDeviceInterpolator: the DeviceInterpolator of a committed scene's (buffer type, slot) (all zero, with the
+        error recorded, when it is refused)."""
+        ip = DeviceInterpolator()
+        self.rtcb200GetSceneDeviceInterpolator(scene, buffer_type, slot, C.byref(ip))
+        return ip
 
     def scene_arrays(self, scene):
         """Copy of a committed scene's acceleration structure (rtcb200CopySceneArrays), for inspection: dict of the layout fields

@@ -488,10 +488,54 @@ struct RTCB200DeviceTraversable {
   unsigned short general;    /* records index `descs` */
   short device;              /* CUDA ordinal of the scene's device */
   unsigned int curves;       /* 2: curve records among them, 1: point records only */
-  const struct RTCB200DeviceGeometry* geometries;   /* indexed like `descs` (by geomID when `descs` is NULL); NULL: empty scene */
+  const struct RTCB200DeviceGeometry* geometries;   /* indexed like `descs` (by geomID when `descs` is NULL), with an
+                                                       RTCB200DeviceGeometryHeader in front of entry 0; NULL: a scene without
+                                                       geometries */
 };   /* 48 bytes, the fields the queries read at fixed offsets: kernels take the struct by value, and a larger parameter would
       change the code of every kernel that traces, filters or not */
 RTCB200_API void rtcb200GetSceneDeviceTraversable(RTCScene scene, struct RTCB200DeviceTraversable* out);
+/* The same snapshot, indexed by geomID, for the shading getters of embree4_b200_device.cuh
+ * (rtcb200GetGeometryUserDataFromTraversable / rtcb200GetGeometryTransformFromTraversable): one entry per geomID of the scene. */
+struct RTCB200DeviceGeometryInfo {
+  void* userPtr;                   /* rtcSetGeometryUserData of the geometry itself (an instance's own); NULL for an empty slot */
+  unsigned int isInstance;         /* RTC_GEOMETRY_TYPE_INSTANCE */
+  float xfm[12];                   /* an instance's local-to-world columns vx | vy | vz | p; zero for other geometries */
+};   /* 64 bytes */
+/* The 16 bytes in front of geometries[0]: the geomID block of the same allocation and its number of entries. */
+struct RTCB200DeviceGeometryHeader {
+  const struct RTCB200DeviceGeometryInfo* byGeomID;
+  unsigned int count;
+  unsigned int reserved;
+};
+
+/* Interpolating vertex data from the caller's own CUDA kernels: rtcb200Interpolate1 (embree4_b200_device.cuh) runs, for one hit,
+ * the body rtcb200InterpolateHitsDevice runs for every hit of a batch, with the same results bit for bit.
+ *  - rtcb200GetSceneDeviceInterpolator fills `out` with the scene's interpolation table for (type, slot): the very table the
+ *    batched calls use, built by the first request after a commit -- batched or this getter -- and shared by both.  It uploads
+ *    the buffers as their host contents are at that moment (the batched calls' rule).  The build runs on a stream of the calling
+ *    thread's own and is complete when the getter returns.
+ *  - Refused, with RTC_ERROR_INVALID_OPERATION recorded, `*out` zeroed and nothing launched: an uncommitted or modified scene, and a
+ *    buffer type other than RTC_BUFFER_TYPE_VERTEX (slot 0) or RTC_BUFFER_TYPE_VERTEX_ATTRIBUTE.
+ *  - Valid until the scene's next rtcCommitScene or its final release: kernels that use it must have completed before either.
+ *    Use it on the scene's CUDA device.  Its fields are not part of the interface. */
+struct RTCB200DeviceInterpolator {
+  const void* table;         /* device table: the scene's geometries, then one block per instanced scene */
+  unsigned int nentries;     /* entries of the scene's own geometries */
+  unsigned int reserved;
+};
+/* rtcb200Interpolate1's arguments: RTCInterpolateArguments with the geometry given as a hit names it, and no buffer (the
+ * interpolator has it).  geomID RTC_INVALID_GEOMETRY_ID (a miss) writes nothing; instID not RTC_INVALID_GEOMETRY_ID means geometry
+ * geomID of the scene that instance instID of the interpolator's scene instantiates (a hit's instID[0]).  Value k of each output
+ * goes to P[k], dPdu[k], ... as rtcInterpolate writes it; NULL outputs are skipped.  valueCount must not exceed the floats the
+ * buffer's format holds. */
+struct RTCB200DeviceInterpolateArguments {
+  unsigned int geomID, instID, primID;
+  float u, v;
+  float *P, *dPdu, *dPdv, *ddPdudu, *ddPdvdv, *ddPdudv;
+  unsigned int valueCount;
+};
+RTCB200_API void rtcb200GetSceneDeviceInterpolator(RTCScene scene, enum RTCBufferType type, unsigned int slot,
+                                                   struct RTCB200DeviceInterpolator* out);
 
 /* =====================================================================================================
  * Section C -- the rest of the reference library's export list (kernels/export.linux.map: every rtc* symbol).

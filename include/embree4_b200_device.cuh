@@ -50,9 +50,35 @@
 //  - Candidates come in traversal order, one per leaf record (a sphere point's back hit, or a second root of a curve segment,
 //    is not offered after its front hit is rejected).  Geometry filter callbacks never run on the device.
 //  - The scene flag RTC_SCENE_FLAG_FILTER_FUNCTION_IN_ARGUMENTS is not required, as on the host.
+//
+// Shading at a hit, in the same kernel (Embree 4's rtcGetGeometryUserDataFromTraversable / rtcGetGeometryTransformFromTraversable
+// in SYCL device code, rtcore_scene.h:247,250, and rtcInterpolate through a table of the scene's buffers):
+//
+//   __global__ void shade(RTCB200DeviceTraversable t, RTCB200DeviceInterpolator normals, ...) {   // normals: VERTEX_ATTRIBUTE slot
+//     rtcb200TraversableIntersect1(t, &rh);
+//     if (rh.hit.geomID == RTC_INVALID_GEOMETRY_ID) return;
+//     float n[3];
+//     RTCB200DeviceInterpolateArguments ia = {rh.hit.geomID, rh.hit.instID[0], rh.hit.primID, rh.hit.u, rh.hit.v, n};
+//     ia.valueCount = 3;
+//     rtcb200Interpolate1(normals, &ia);                  // object space
+//     float x[12];
+//     rtcb200GetGeometryTransformFromTraversable(t, rh.hit.instID[0], 0.0f, RTC_FORMAT_FLOAT3X4_COLUMN_MAJOR, x);   // identity when
+//     ...                                                  // the hit is not instanced
+//   }
+//
+//  - rtcb200GetGeometryUserDataFromTraversable(t, geomID): the user data of geometry geomID of the traversable's own scene (an
+//    instance's own pointer for an instance); NULL for an id beyond the scene's geometries or an empty slot.
+//  - rtcb200GetGeometryTransformFromTraversable: an instance's local-to-world transform, in the bytes the host
+//    rtcGetGeometryTransformFromScene writes for RTC_FORMAT_FLOAT3X4_ROW_MAJOR, _FLOAT3X4_COLUMN_MAJOR or _FLOAT4X4_COLUMN_MAJOR;
+//    identity for any other geometry or an invalid id; `time` is ignored (one time step); another format leaves xfm untouched.
+//  - Both read the snapshot rtcb200GetSceneDeviceTraversable took: user data and transforms as they were at that call.
+//  - rtcb200Interpolate1: see RTCB200DeviceInterpolateArguments (embree4_b200.h).  Points, instances, a missing buffer or slot, and
+//    a primitive or element beyond its buffer write quiet NaN, as the batched call does.
 #pragma once
 #include "embree4_b200.h"
 #include "../embree_b200/csrc/record_tests.cuh"
+#include "../embree_b200/csrc/interp.cuh"
+#include "../embree_b200/csrc/transform_format.cuh"
 
 namespace rtk {
 
@@ -316,6 +342,27 @@ __device__ __forceinline__ void device_query1_dispatch(const RTCB200DeviceTraver
   }
 }
 
+// entry geomID of the snapshot's geomID block (the header in front of t.geometries[0] locates it), or NULL
+__device__ __forceinline__ const RTCB200DeviceGeometryInfo* geometry_info(const RTCB200DeviceTraversable& t, unsigned geomID) {
+  if (!t.geometries) return nullptr;
+  const RTCB200DeviceGeometryHeader* h = reinterpret_cast<const RTCB200DeviceGeometryHeader*>(t.geometries) - 1;
+  return geomID < h->count ? h->byGeomID + geomID : nullptr;
+}
+
+// One hit of rtcb200InterpolateHitsDevice, its value k written at index k.  A function of its own, so the caller's kernel does not
+// carry the interpolation's registers through its other code.
+inline __device__ __noinline__ void device_interpolate1(const RTCB200DeviceInterpolator ip, const RTCB200DeviceInterpolateArguments* a) {
+  const uint32_t geomID = a->geomID;
+  if (geomID == kInvalidID) return;   // a miss: nothing is written
+  float* const out[6] = {a->P, a->dPdu, a->dPdv, a->ddPdudu, a->ddPdvdv, a->ddPdudv};
+  interpolate_hit(static_cast<const InterpEntry*>(ip.table), ip.nentries, geomID, a->instID, a->primID, a->u, a->v, a->valueCount,
+                  [&](unsigned k, const float o[6]) {
+#pragma unroll
+                    for (int c = 0; c < 6; ++c)
+                      if (out[c]) out[c][k] = o[c];
+                  });
+}
+
 }  // namespace rtk
 
 // Closest hit of one ray: as one record of rtcb200Intersect1MDevice.  No filter code is compiled in: args->filter is not called.
@@ -338,4 +385,26 @@ __device__ __forceinline__ void rtcb200TraversableIntersect1(const RTCB200Device
 template <unsigned FEATURES>
 __device__ __forceinline__ void rtcb200TraversableOccluded1(const RTCB200DeviceTraversable& t, RTCRay* ray, const RTCOccludedArguments* args) {
   rtk::device_query1_dispatch<true, FEATURES>(t, ray, nullptr, args);
+}
+
+// User data of geometry geomID of the traversable's scene (rtcore_sycl.cpp:114-118); NULL for an invalid id or an empty slot.
+__device__ __forceinline__ void* rtcb200GetGeometryUserDataFromTraversable(const RTCB200DeviceTraversable& t, unsigned int geomID) {
+  const RTCB200DeviceGeometryInfo* e = rtk::geometry_info(t, geomID);
+  return e ? e->userPtr : nullptr;
+}
+// Local-to-world transform of instance geomID, identity for any other geometry or an invalid id (rtcore_sycl.cpp:120-133); the
+// bytes of the host rtcGetGeometryTransformFromScene.  An unknown format leaves xfm untouched.
+__device__ __forceinline__ void rtcb200GetGeometryTransformFromTraversable(const RTCB200DeviceTraversable& t, unsigned int geomID, float time,
+                                                                           enum RTCFormat format, void* xfm) {
+  (void)time;   // one time step
+  const RTCB200DeviceGeometryInfo* e = rtk::geometry_info(t, geomID);
+  float m[12] = {1.0f, 0.0f, 0.0f, 0.0f, 1.0f, 0.0f, 0.0f, 0.0f, 1.0f, 0.0f, 0.0f, 0.0f};
+  if (e && e->isInstance)
+    for (int k = 0; k < 12; ++k) m[k] = e->xfm[k];
+  rtk::store_transform(m, (unsigned)format, static_cast<float*>(xfm));
+}
+// rtcInterpolate of one hit through a scene's interpolator (rtcb200GetSceneDeviceInterpolator): the values
+// rtcb200InterpolateHitsDevice writes for the same hit, value k of each output at index k.
+__device__ __forceinline__ void rtcb200Interpolate1(const RTCB200DeviceInterpolator& ip, const RTCB200DeviceInterpolateArguments* args) {
+  rtk::device_interpolate1(ip, args);
 }
