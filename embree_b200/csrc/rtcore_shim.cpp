@@ -767,7 +767,6 @@ rtk::TraceParams make_params(SceneImpl* s, void* rays, const int* valid, unsigne
   p.nodes = s->gpu.nodes; p.tris = s->gpu.tris; p.root_valid = s->gpu.root_valid; p.robust = s->gpu.robust;
   p.descs = s->gpu.general ? s->gpu.d_descs : nullptr;
   p.curves = s->gpu.curves;
-  p.top_nodes = s->gpu.levels.size() > 3 ? s->gpu.levels[3] : s->gpu.num_nodes;
   p.rays = rays; p.valid = valid; p.n = n; p.instID = instID; p.instPrimID = instPrimID;
   p.stat = s->statCounters ? s->gpu.d_stat : nullptr;
   return p;

@@ -146,7 +146,6 @@ struct TraceParams {
   int tri_batch_min = 8, tri_wait_max = 4, refill_min = 4, use_prefetch = 1;  // filled by launch_trace from tuning()
   const GeomDesc* descs = nullptr;  // non-NULL: instanced scene, record.geomID slot holds a descriptor index
   int curves = 0;                   // the scene holds curve or point records (descs != NULL): 2 curves among them, 1 points only
-  uint32_t top_nodes = 0;           // nodes in the first three BVH8 levels (RTK_TOP_SMEM experiment)
   int robust = 0;  // scene built with RTC_SCENE_FLAG_ROBUST: triangle records hold v0,v1,v2, Pluecker test
   // filter-callback passes (K == 1 closest hit): per-ray lists of rejected record indices (excl_off has n + 1 entries) and
   // the per-ray output of the winning record index (0xFFFFFFFF on a miss)
