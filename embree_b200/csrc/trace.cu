@@ -411,7 +411,8 @@ __global__ void __launch_bounds__(TRACE_THREADS, RTK_MIN_BLOCKS) trace_kernel(co
         // one of its own while the others idle: on the headline stream about half as many triangle steps, each with about
         // twice as many busy lanes.  Owners queue (record index, owner lane) in shared memory; worker lane w takes item w, fetches the
         // owner's ray by shuffles and tests the record; hits meet in a 64-bit atomicMin per owner keyed by (t, item) --
-        // among equal t the later item wins, as in the sequential order -- and the owner reads u, v back by shuffle.
+        // among equal t (-0 and +0 included) the later item wins, as in the sequential order -- and the owner reads t, u, v
+        // back by shuffle.
         __shared__ uint32_t s_tri[TRACE_WARPS][32];
         __shared__ uint32_t s_owner[TRACE_WARPS][32];
         __shared__ unsigned long long s_best[TRACE_WARPS][32];
@@ -450,7 +451,7 @@ __global__ void __launch_bounds__(TRACE_THREADS, RTK_MIN_BLOCKS) trace_kernel(co
         const float o_tfar = RAY_TFAR(ot);
         const float o_best = __shfl_sync(FULL, tfar_tri, owner);
         const uint32_t o_mask = RAY_MASK(ot);
-        float w_u = 0.0f, w_v = 0.0f;
+        float w_t = 0.0f, w_u = 0.0f, w_v = 0.0f;
         unsigned long long key = ~0ull;
         if (work) {
           const uint4* tp = tris + (size_t)ti * 3;
@@ -466,8 +467,10 @@ __global__ void __launch_bounds__(TRACE_THREADS, RTK_MIN_BLOCKS) trace_kernel(co
             const float rcpAbsDen = 1.0f / th.absDen;
             const float t = th.T * rcpAbsDen;
             if (t <= o_best) {
-              w_u = th.U * rcpAbsDen; w_v = th.V * rcpAbsDen;
-              uint32_t tb32 = __float_as_uint(t);
+              w_t = t; w_u = th.U * rcpAbsDen; w_v = th.V * rcpAbsDen;
+              // t <= best holds between -0 and +0 both ways, so the two zeros must share a key for the later item to win: the
+              // key is made from t + 0 (-0 + 0 = +0), and the winner's own t, sign included, comes from its lane below
+              uint32_t tb32 = __float_as_uint(__fadd_rn(t, 0.0f));
               tb32 ^= (tb32 >> 31) ? 0xFFFFFFFFu : 0x80000000u;   // order-preserving float -> uint
               key = ((unsigned long long)tb32 << 32) | (uint32_t)(31 - lane);
               atomicMin(&s_best[wi][owner], key);
@@ -479,12 +482,10 @@ __global__ void __launch_bounds__(TRACE_THREADS, RTK_MIN_BLOCKS) trace_kernel(co
         const unsigned long long best = s_best[wi][lane];       // as owner
         const bool got = isT && best != ~0ull;
         const int win = got ? 31 - (int)(best & 31ull) : lane;  // worker lane that holds the winning item
-        const float b_u = __shfl_sync(FULL, w_u, win), b_v = __shfl_sync(FULL, w_v, win);
+        const float b_t = __shfl_sync(FULL, w_t, win), b_u = __shfl_sync(FULL, w_u, win), b_v = __shfl_sync(FULL, w_v, win);
         if (got && OCCLUDED) { found = true; ngy = 0; tgy = 0; sp = 0; top_y = 0; }
         else if (got) {
-          uint32_t tb32 = (uint32_t)(best >> 32);
-          tb32 ^= (tb32 >> 31) ? 0x80000000u : 0xFFFFFFFFu;     // inverse of the transform above
-          tfar_tri = __uint_as_float(tb32);
+          tfar_tri = b_t;
           hit_u = b_u; hit_v = b_v; hit_tri = s_tri[wi][win];
           found = true;
         }

@@ -524,3 +524,61 @@ def point_edge_cases(seed=77):
     rays["tnear"] = np.array(tn, np.float32)
     rays["tfar"] = np.maximum(np.array(tf, np.float32), rays["tnear"])
     return pv, pn, rays
+
+
+def signed_zero_grid(cells=8, h=0.25, seed=21):
+    """A planar grid of `cells` x `cells` squares in z = 0, two triangles per square on the same diagonal, the winding flipped
+    from square to square, and rays whose origins lie exactly on its vertices and edges (axis-parallel and diagonal; every
+    coordinate a dyadic fraction, so the triangle test sees them exactly).  Each origin gets an oblique direction into each
+    half-space.  tnear = -1: the triangles around the origin accept t = +0 or -0 (the sign follows from the rounding of the
+    test's cross products), so a ray meets several candidates at the same zero distance; every 7th ray has tnear = 0, where
+    no zero-distance hit may be reported.  Returns (vertices, triangles, rays); the ray count is not a multiple of 32."""
+    from embree_b200.rtc import make_rayhits
+    n = cells
+    ii, jj = np.meshgrid(np.arange(n + 1), np.arange(n + 1), indexing="ij")
+    v = np.stack([ii.ravel() * h, jj.ravel() * h, np.zeros((n + 1) ** 2)], 1).astype(np.float32)
+    tris = []
+    for i in range(n):
+        for j in range(n):
+            a, b = i * (n + 1) + j, (i + 1) * (n + 1) + j
+            c, d = b + 1, a + 1
+            tris += [(a, b, c), (a, c, d)] if (i + j) % 2 == 0 else [(a, c, b), (a, d, c)]
+    s = np.arange(1, 8) * (h / 8)
+    org = [np.stack([ii.ravel() * h, jj.ravel() * h], 1)]                                        # vertices
+    for i in range(n + 1):
+        for j in range(n):
+            org.append(np.stack([np.full(7, i * h), j * h + s], 1))                               # edges along y
+            org.append(np.stack([j * h + s, np.full(7, i * h)], 1))                               # edges along x
+    for i in range(n):
+        for j in range(n):
+            org.append(np.stack([i * h + s, j * h + s], 1))                                       # the diagonals
+    o2 = np.concatenate(org, 0)
+    o = np.concatenate([o2, np.zeros((len(o2), 1))], 1).astype(np.float32)
+    o = np.repeat(o, 2, axis=0)
+    rng = np.random.RandomState(seed)
+    d = np.concatenate([rng.uniform(-1, 1, (len(o), 2)), rng.uniform(0.2, 1.0, (len(o), 1))], 1)
+    d[1::2, 2] *= -1                                                                               # both half-spaces
+    rays = make_rayhits(o, d.astype(np.float32), tnear=-1.0)
+    rays["tnear"][::7] = 0.0
+    assert len(rays) % 32 != 0
+    return v, np.array(tris, np.uint32), rays
+
+
+def zero_distance_candidates(v, t, rays):
+    """Moeller-Trumbore in float64 for every (ray, triangle) pair of a small scene: [rays, triangles] boolean of the triangles whose
+    closed triangle contains the ray's origin (t = 0, u >= 0, v >= 0, u + v <= 1, non-parallel)."""
+    V = v.astype(np.float64)
+    v0, v1, v2 = V[t[:, 0]], V[t[:, 1]], V[t[:, 2]]
+    e1, e2 = v1 - v0, v2 - v0
+    O = np.stack([rays["org_x"], rays["org_y"], rays["org_z"]], 1).astype(np.float64)[:, None, :]
+    D = np.stack([rays["dir_x"], rays["dir_y"], rays["dir_z"]], 1).astype(np.float64)[:, None, :]
+    p = np.cross(D, e2[None])
+    det = (e1[None] * p).sum(-1)
+    sv = O - v0[None]
+    q = np.cross(sv, e1[None])
+    with np.errstate(divide="ignore", invalid="ignore"):
+        uu = (sv * p).sum(-1) / det
+        vv = (D * q).sum(-1) / det
+        tt = (e2[None] * q).sum(-1) / det
+    eps = 1e-12
+    return (det != 0) & (np.abs(tt) <= eps) & (uu >= -eps) & (vv >= -eps) & (uu + vv <= 1 + eps)

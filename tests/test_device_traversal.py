@@ -3,7 +3,8 @@
 CPU: a user translation unit that includes only the public headers compiles for sm_90a with -I include, and two of them
 device-link with -rdc=true.  GPU: tests/device_api/devtrace.cu traces from device code and every byte of every record (misses
 included) must equal what rtcb200Intersect1MDevice / rtcb200Occluded1MDevice write for a copy of the same input, over triangle,
-quad, instanced, curve, point, two-level, refitted and empty scenes; plus the getter's refusals."""
+quad, instanced, curve, point, two-level, refitted and empty scenes, and for rays whose candidates tie at t = +0 / -0; plus the
+getter's refusals."""
 import ctypes as C
 import os
 import subprocess
@@ -281,6 +282,23 @@ def test_two_level_and_refitted_dynamic_scenes(b200, devtrace):
     lib.check(dev)
     assert lib.scene_stats(sc).builder == 2
     compare_queries(lib, dev, devtrace, sc, query_rays(N_RAYS, (0, 0, 0), 2.5, seed=9))
+    _release(lib, sc)
+
+
+@pytest.mark.gpu
+def test_signed_zero_distance_ties(b200, devtrace):
+    """Origins exactly on a planar grid with tnear < 0: each ray meets several candidates at t = +0 or -0, and the device query
+    must pick the same winner as the batched kernels' warp-wide triangle step (the later candidate, the two zeros being equal)."""
+    from tests.parity import signed_zero_grid
+    lib, dev = b200
+    v, t, rh = signed_zero_grid()
+    sc = lib.rtcNewScene(dev)
+    _, keep = lib.add_triangle_mesh(dev, sc, v, t, mask=0xFFFFFFFF)
+    lib.rtcCommitScene(sc)
+    lib.check(dev)
+    out = compare_queries(lib, dev, devtrace, sc, rh)
+    neg = rh["tnear"] < 0
+    assert (out["geomID"][neg] == 0).all() and ((out["tfar"][neg].view(np.uint32) & 0x7FFFFFFF) == 0).all()
     _release(lib, sc)
 
 

@@ -67,36 +67,3 @@ def test_gather_empty_scene_writes_miss_records(b200):
     assert torch.equal(out[:, 0], rays[:, 8]) and (out[:, 1:6] == 0).all() and (out.view(torch.int32)[:, 6:8] == -1).all()
     lib.rtcReleaseScene(sc)
 
-
-@pytest.mark.skipif(not __import__("os").environ.get("RTCB200_TEST_SPREAD"), reason="experimental kernel variant: set RTCB200_TEST_SPREAD=1")
-def test_tri_spread_matches_default(b200):
-    """The opt-in warp-wide triangle redistribution (trace.cu SPREAD, "tri_spread" 1) must report the same hits as the
-    default kernel: ids identical except equal-distance ties, t/u/v bit-equal for the same primitive."""
-    import numpy as np
-    import torch
-    from tests.parity import compare_hits
-    lib, dev = b200
-    v, t = scenes.triangle_sphere(300)
-    sc, keep = build_scene(lib, dev, [(v, t, 0, 0xFFFFFFFF)])
-    prim = scenes.primary_rays(640, 360, eye=(0.15, -0.1, 0.05), look=(0.3, 0.2, 1.0), device=torch.device("cuda", 0))
-    a = lib.args()
-    st = torch.cuda.current_stream().cuda_stream
-    lib.rtcb200Intersect1MDevice(sc, C.c_void_p(prim.data_ptr()), prim.shape[0], C.byref(a), C.c_void_p(st))
-    rays = scenes.diffuse_bounce_rays(prim, seed=1, replicate=8)
-    out = []
-    try:
-        for spread in (0, 1):
-            assert lib.rtcb200SetTuning(b"tri_spread", spread) == 0
-            B = rays.clone()
-            lib.rtcb200Intersect1MDevice(sc, C.c_void_p(B.data_ptr()), B.shape[0], C.byref(a), C.c_void_p(st))
-            torch.cuda.synchronize()
-            lib.check(dev)
-            out.append(scenes.as_numpy_rayhits(B.cpu()))
-    finally:
-        lib.rtcb200SetTuning(b"tri_spread", 0)
-    rep = compare_hits(out[0], out[1], 1e-6)
-    assert rep["hits"] > 1000000 and rep["id_mismatch"] == 0 and rep["hit_miss_disagree"] == 0 and rep["tie"] <= 50, rep
-    same = (out[0]["primID"] == out[1]["primID"]) & (out[0]["geomID"] != 0xFFFFFFFF)
-    for f in ("tfar", "u", "v", "Ng_x", "Ng_y", "Ng_z"):
-        assert (out[0][f].view(np.uint32) == out[1][f].view(np.uint32))[same].all(), f
-    lib.rtcReleaseScene(sc)
