@@ -53,10 +53,8 @@ struct LargeScratch {
   uint32_t chunk0;                       // first chunk id of this task
 };
 
-__device__ __forceinline__ int f2o(float f) { int i = __float_as_int(f); return i >= 0 ? i : i ^ 0x7FFFFFFF; }
-__device__ __forceinline__ float o2f(int i) { return __int_as_float(i >= 0 ? i : i ^ 0x7FFFFFFF); }
-constexpr int kOrdPosInf = 0x7F800000;            // f2o(+inf)
-constexpr int kOrdNegInf = (int)0x807FFFFF;       // f2o(-inf)
+constexpr int kOrdPosInf = 0x7F800000;            // f2ord(+inf)
+constexpr int kOrdNegInf = (int)0x807FFFFF;       // f2ord(-inf)
 
 struct BinMap { float lo[3], scale[3]; };
 __device__ __forceinline__ BinMap make_map(const float clo[3], const float chi[3]) {
@@ -87,7 +85,7 @@ __device__ __forceinline__ SweepResult sweep_axis(const int* lo /*[kBins][3]*/, 
   const int lane = threadIdx.x & 31;
   float b[6];
 #pragma unroll
-  for (int k = 0; k < 3; ++k) { b[k] = o2f(lo[lane * 3 + k]); b[3 + k] = o2f(hi[lane * 3 + k]); }
+  for (int k = 0; k < 3; ++k) { b[k] = ord2f(lo[lane * 3 + k]); b[3 + k] = ord2f(hi[lane * 3 + k]); }
   uint32_t c = cnt[lane];
   // inclusive prefix (left) and suffix (right) of boxes / counts
   float L[6], R[6];
@@ -271,7 +269,7 @@ __global__ void __launch_bounds__(NT* GROUPS) sah_group_kernel(const SahTask* __
         packed |= (uint32_t)b << (5 * a);
         atomicAdd(&gs->cnt[a][b], 1u);
 #pragma unroll
-        for (int k = 0; k < 3; ++k) { atomicMin(&gs->lo[a][b][k], f2o(lo[k])); atomicMax(&gs->hi[a][b][k], f2o(hi[k])); }
+        for (int k = 0; k < 3; ++k) { atomicMin(&gs->lo[a][b][k], f2ord(lo[k])); atomicMax(&gs->hi[a][b][k], f2ord(hi[k])); }
       }
       sid[i] = id; sbin[i] = packed;
     }
@@ -332,7 +330,7 @@ __global__ void __launch_bounds__(NT* GROUPS) sah_group_kernel(const SahTask* __
         const int s = left ? 0 : 1;
 #pragma unroll
         for (int k = 0; k < 3; ++k) {
-          const int c = f2o(lo3[k] + hi3[k]);
+          const int c = f2ord(lo3[k] + hi3[k]);
           flo[s][k] = min(flo[s][k], c); fhi[s][k] = max(fhi[s][k], c);
         }
       }
@@ -365,8 +363,8 @@ __global__ void __launch_bounds__(NT* GROUPS) sah_group_kernel(const SahTask* __
       for (int k = 0; k < 6; ++k) { lb[k] = gs->lbox[k]; rb[k] = gs->rbox[k]; }
 #pragma unroll
       for (int k = 0; k < 3; ++k) {
-        lcl[k] = o2f(gs->c_lo[0][k]); lch[k] = o2f(gs->c_hi[0][k]);
-        rcl[k] = o2f(gs->c_lo[1][k]); rch[k] = o2f(gs->c_hi[1][k]);
+        lcl[k] = ord2f(gs->c_lo[0][k]); lch[k] = ord2f(gs->c_hi[0][k]);
+        rcl[k] = ord2f(gs->c_lo[1][k]); rch[k] = ord2f(gs->c_hi[1][k]);
       }
       if (dim < 0) {
         // all centres coincide (or NaN-free degenerate): both children get the parent's box, which is conservative
@@ -437,7 +435,7 @@ __global__ void __launch_bounds__(256) sah_large_bin(const SahTask* __restrict__
       const int b = bin_of(map, lo[a] + hi[a], a);
       atomicAdd(&scnt[a][b], 1u);
 #pragma unroll
-      for (int k = 0; k < 3; ++k) { atomicMin(&slo[a][b][k], f2o(lo[k])); atomicMax(&shi[a][b][k], f2o(hi[k])); }
+      for (int k = 0; k < 3; ++k) { atomicMin(&slo[a][b][k], f2ord(lo[k])); atomicMax(&shi[a][b][k], f2ord(hi[k])); }
     }
   }
   __syncthreads();
@@ -516,7 +514,7 @@ __global__ void __launch_bounds__(256) sah_large_partition(const SahTask* __rest
       left[j] = dim >= 0 ? bin_of(map, c[dim], dim) < pos : (i - t.begin) < nl;
       const int sd = left[j] ? 0 : 1;
 #pragma unroll
-      for (int k = 0; k < 3; ++k) { const int o = f2o(c[k]); flo[sd][k] = min(flo[sd][k], o); fhi[sd][k] = max(fhi[sd][k], o); }
+      for (int k = 0; k < 3; ++k) { const int o = f2ord(c[k]); flo[sd][k] = min(flo[sd][k], o); fhi[sd][k] = max(fhi[sd][k], o); }
       if (left[j]) ++myl; else ++myr;
     }
   }
@@ -569,7 +567,7 @@ __global__ void __launch_bounds__(128) sah_large_emit(const SahTask* __restrict_
   const LargeScratch& s = scr[ti];
   float lb[6], rb[6], lcl[3], lch[3], rcl[3], rch[3];
   for (int k = 0; k < 6; ++k) { lb[k] = s.lbox[k]; rb[k] = s.rbox[k]; }
-  for (int k = 0; k < 3; ++k) { lcl[k] = o2f(s.lc_lo[k]); lch[k] = o2f(s.lc_hi[k]); rcl[k] = o2f(s.rc_lo[k]); rch[k] = o2f(s.rc_hi[k]); }
+  for (int k = 0; k < 3; ++k) { lcl[k] = ord2f(s.lc_lo[k]); lch[k] = ord2f(s.lc_hi[k]); rcl[k] = ord2f(s.rc_lo[k]); rch[k] = ord2f(s.rc_hi[k]); }
   if (s.dim < 0) {
     const Node2& self = nodes[t.node];
     lb[0] = rb[0] = self.lox; lb[1] = rb[1] = self.loy; lb[2] = rb[2] = self.loz;

@@ -823,6 +823,8 @@ RT_HD int sweep_select_min(uint32_t valid, const float* v) {
   for (int i = 0; i < kSweepW; ++i) if ((valid >> i) & 1u) if (best < 0 || v[i] < v[best]) best = i;
   return best;
 }
+// first-level sub-segments of the sweep: the BVH primitives of one round cubic curve (rtk_device.h prims_per_curve)
+constexpr int kRoundSubSegs = kSweepW - 1;
 // `lane` >= 0 restricts the FIRST subdivision level to that one of its 7 sub-segments: the BVH holds every first-level
 // sub-segment of a round curve as its own primitive (tight boxes), and the closest hit over them is the closest hit of the curve
 // (the same converged roots; only the order in which candidates shorten the ray differs).  lane < 0: the whole curve.

@@ -452,10 +452,11 @@ struct CommitUpload {
     if (rtk::curve_record(pt.kind)) {
       // cubic curves (scene_curves.cpp): float4 control vertices, one index per curve (first control vertex), Hermite adds float4
       // tangents; the basis weights at the tessellation points are tabulated here as the reference tabulates them
-      const bool hermite = is_hermite(g->type), round = pt.kind == rtk::PRIM_ROUND_CUBIC;
+      const bool hermite = is_hermite(g->type);
       if (hermite && !g->tangents.buf) fail(RTC_ERROR_INVALID_OPERATION, "tangent buffer not set");
       if (hermite && g->tangents.count != nverts) fail(RTC_ERROR_INVALID_OPERATION, "number of tangents must match number of vertices");   // scene_curves.cpp commit
-      const size_t segs = round ? 7 : (size_t)g->tessellationRate;   // BVH primitives per curve: the 7 first-level sub-segments of the sweep / the ribbon's segments
+      d.tess = (uint32_t)g->tessellationRate;
+      const size_t segs = rtk::prims_per_curve(d);
       if (nprims * segs > 0x7FFFFFFFull || nverts > 0xFFFFFFFFull) fail(RTC_ERROR_INVALID_OPERATION, "curve geometry too large");
       d.verts = copy(g->vertices.data(), curveVertBytes, true, "curve vertices");
       s->residentCurves[g].verts = d.verts;
@@ -466,12 +467,11 @@ struct CommitUpload {
         d.tstride = g->tangents.stride; d.hermite = 1;
       }
       d.basis = pt.basis;
-      d.tess = (uint32_t)g->tessellationRate;
       float tab[8 * (rtk::kMaxTess + 1)];
       rtk::curve_basis_table(d.basis, g->tessellationRate, tab);
       d.basis_tab = reinterpret_cast<const float*>(copy(tab, sizeof(float) * 8 * (g->tessellationRate + 1), true, "curve basis table"));
       cuda_check(cudaStreamSynchronize(0), "upload curve basis table");   // `tab` is on the stack
-      d.ntris = (uint32_t)(nprims * segs);   // flat: one BVH primitive per tessellation segment; round: per first-level sub-segment of the sweep intersector
+      d.ntris = (uint32_t)(nprims * segs);
       return true;
     }
     const bool quad = g->type == RTC_GEOMETRY_TYPE_QUAD;

@@ -59,7 +59,15 @@ struct GeomDesc {
   float w2l[12] = {1, 0, 0, 0, 1, 0, 0, 0, 1, 0, 0, 0};
 };
 
+// BVH primitives per curve of a cubic curve geometry: the sweep's first-level sub-segments (round) or the ribbon's tessellation
+// segments (flat).  Primitive `curve * prims_per_curve + segment` is that segment of that curve.
+RT_HD uint32_t prims_per_curve(const GeomDesc& g) { return g.kind == PRIM_ROUND_CUBIC ? (uint32_t)kRoundSubSegs : g.tess; }
+
 #if defined(__CUDACC__)
+// float <-> int mapping that orders like the floats, so that atomicMin / atomicMax on ints reduce boxes (build.cu, build_sah.cu)
+__device__ __forceinline__ int f2ord(float f) { int i = __float_as_int(f); return i >= 0 ? i : i ^ 0x7FFFFFFF; }
+__device__ __forceinline__ float ord2f(int i) { return __int_as_float(i >= 0 ? i : i ^ 0x7FFFFFFF); }
+
 // the four control points of the flat cubic curve whose index-buffer entry is `vid` (CurveGeometry::gather,
 // scene_curves.h:107-113; Hermite: HermiteCurveT's conversion to Bezier control points, hermite_curve.h:19-20)
 __device__ __forceinline__ void load_cubic_cp(const GeomDesc& g, uint32_t vid, CurveVtx cp[4]) {
