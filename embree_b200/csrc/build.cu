@@ -1044,6 +1044,29 @@ int refit_scene(SceneGPU& s, const GeomDesc* geoms, int ngeoms, cudaStream_t st,
 
 
 // ---------------------------------------------------------------------------------------------------
+// linear curves: one neighbour-flag byte per segment (LineSegments::commit, scene_line_segments.cpp:209-232)
+// ---------------------------------------------------------------------------------------------------
+// The application's flags & 3 when it set a flags buffer, otherwise derived from the index buffer: a segment has a right neighbour
+// when the next segment starts at its end vertex, and a left one when the previous segment ends at its start vertex.
+__global__ void __launch_bounds__(256) curve_flags(const uint8_t* __restrict__ idx, uint64_t istride, const uint8_t* __restrict__ app,
+                                                   uint64_t fstride, uint32_t n, uint8_t* __restrict__ out) {
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  if (app) { out[i] = app[(uint64_t)i * fstride] & 3u; return; }
+  const uint32_t cur = __ldg(reinterpret_cast<const uint32_t*>(idx + (uint64_t)i * istride));
+  const bool left = i > 0 && __ldg(reinterpret_cast<const uint32_t*>(idx + (uint64_t)(i - 1) * istride)) + 1u == cur;
+  const bool right = i + 1 < n && __ldg(reinterpret_cast<const uint32_t*>(idx + (uint64_t)(i + 1) * istride)) == cur + 1u;
+  out[i] = (uint8_t)((left ? 1u : 0u) | (right ? 2u : 0u));   // RTC_CURVE_FLAG_NEIGHBOR_LEFT | _RIGHT
+}
+
+int linear_curve_flags(const uint8_t* idx, uint64_t istride, const uint8_t* app, uint64_t fstride, uint32_t n, uint8_t* out, cudaStream_t st) {
+  if (n == 0) return 0;
+  curve_flags<<<(n + 255) / 256, 256, 0, st>>>(idx, istride, app, fstride, n, out);
+  count_launch();
+  return (int)cudaGetLastError();
+}
+
+// ---------------------------------------------------------------------------------------------------
 // two-level scenes: relocation of a sub-BVH into the scene's arrays + host-built top level (see rtk_device.h)
 // ---------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256) relocate_nodes(const Node8* __restrict__ src, uint32_t n, Node8* __restrict__ dst, uint32_t node_off, uint32_t tri_off) {

@@ -101,6 +101,7 @@ struct BufferImpl : RefCounted {
   char* ptr = nullptr;
   size_t bytes = 0;
   bool shared = false;
+  bool device = false;   // rtcb200SetSharedGeometryBufferDevice: `ptr` is the caller's memory on the library's GPU, not the host's
   BufferImpl(DeviceImpl* d, size_t n, void* user) : dev(d), bytes(n), shared(user != nullptr) {
     dev->retain();
     if (user) ptr = static_cast<char*>(user);
@@ -125,7 +126,10 @@ struct BufferView {
     if (buf) buf->release();
     buf = b; offset = off; stride = st; count = n; format = f;
   }
-  const char* data() const { return buf ? buf->ptr + offset : nullptr; }
+  const char* data() const { return buf && buf->ptr ? buf->ptr + offset : nullptr; }   // NULL: an empty device view
+  bool on_device() const { return buf && buf->device; }
+  // how a device copy of the view's bytes is made
+  cudaMemcpyKind copy_kind() const { return on_device() ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice; }
   ~BufferView() { if (buf) buf->release(); }
 };
 
@@ -369,14 +373,23 @@ struct CommitUpload {
   std::unordered_map<GeometryImpl*, rtk::GeomDesc> uploaded;   // descriptor of every uploaded geometry, before geomID and instance
   explicit CommitUpload(SceneImpl* scene) : s(scene) {}
 
-  // device copy of `bytes` at `src` (nothing to copy: a 16-byte placeholder), freed right after the build or, `resident`, kept for the
-  // trace kernel until the next commit
-  const uint8_t* copy(const void* src, size_t bytes, bool resident, const char* what) {
+  // `bytes` of device memory (at least a 16-byte placeholder), freed right after the build or, `resident`, kept for the trace kernel
+  // until the next commit
+  uint8_t* alloc(size_t bytes, bool resident, const char* what) {
     void* p = nullptr;
     cuda_check(cudaMallocAsync(&p, bytes ? bytes : 16, 0), (std::string("cudaMallocAsync(") + what + ")").c_str());
     (resident ? s->residentBuffers : s->deviceBuffers).push_back(p);
-    if (bytes) cuda_check(cudaMemcpyAsync(p, src, bytes, cudaMemcpyHostToDevice, 0), (std::string("upload ") + what).c_str());
-    return static_cast<const uint8_t*>(p);
+    return static_cast<uint8_t*>(p);
+  }
+  // device copy of `bytes` at `src`, host memory or (`kind` device-to-device) the caller's device memory; the build reads the same
+  // fresh allocation either way
+  const uint8_t* copy(const void* src, size_t bytes, bool resident, const char* what, cudaMemcpyKind kind = cudaMemcpyHostToDevice) {
+    uint8_t* p = alloc(bytes, resident, what);
+    if (bytes) cuda_check(cudaMemcpyAsync(p, src, bytes, kind, 0), (std::string("upload ") + what).c_str());
+    return p;
+  }
+  const uint8_t* copy(const BufferView& v, size_t bytes, bool resident, const char* what) {
+    return v.data() ? copy(v.data(), bytes, resident, what, v.copy_kind()) : alloc(bytes, resident, what);   // an empty device view: nothing to copy
   }
 
   // Adds the descriptor of `g` as `geomID`, seen through the instance `inst` (`instID` in its scene) when that is not null.  False when
@@ -415,9 +428,9 @@ struct CommitUpload {
       if (oriented && !g->tangents.buf) fail(RTC_ERROR_INVALID_OPERATION, "normal buffer not set");
       if (oriented && g->tangents.count != nverts) fail(RTC_ERROR_INVALID_OPERATION, "number of normals must match number of vertices");
       if (nverts > 0x7FFFFFFFull) fail(RTC_ERROR_INVALID_OPERATION, "point geometry too large");
-      d.verts = copy(g->vertices.data(), (nverts - 1) * g->vertices.stride + 16, false, "point vertices");
+      d.verts = copy(g->vertices, (nverts - 1) * g->vertices.stride + 16, false, "point vertices");
       if (oriented) {
-        d.tangents = copy(g->tangents.data(), (nverts - 1) * g->tangents.stride + 12, false, "point normals");
+        d.tangents = copy(g->tangents, (nverts - 1) * g->tangents.stride + 12, false, "point normals");
         d.tstride = g->tangents.stride;
       }
       d.ntris = (uint32_t)nverts;
@@ -429,23 +442,16 @@ struct CommitUpload {
     const size_t curveVertBytes = nverts ? (nverts - 1) * g->vertices.stride + 16 : 16, curveIdxBytes = (nprims - 1) * g->indices.stride + 4;
     if (pt.kind == rtk::PRIM_ROUND_LINEAR || pt.kind == rtk::PRIM_FLAT_LINEAR) {
       // linear curves (scene_line_segments.cpp): one index per segment, neighbour flags from the application or derived from the
-      // index buffer as LineSegments::commit does (:209-232)
+      // index buffer as LineSegments::commit does (:209-232), computed on the device from the copies (rtk::linear_curve_flags)
       if (nprims > 0x3FFFFFFFull || nverts > 0x3FFFFFFFull) fail(RTC_ERROR_INVALID_OPERATION, "curve geometry too large");
       if (g->flags.buf && g->flags.count != nprims) fail(RTC_ERROR_INVALID_OPERATION, "flags buffer must hold one entry per segment");
-      std::vector<unsigned char> fl(nprims);
-      bool hasLeft = false;
-      for (size_t i = 0; i < nprims; ++i) {
-        if (g->flags.buf) { fl[i] = *reinterpret_cast<const unsigned char*>(g->flags.data() + i * g->flags.stride) & 3u; continue; }
-        const unsigned cur = *reinterpret_cast<const unsigned*>(g->indices.data() + i * g->indices.stride);
-        const bool hasRight = (i + 1 < nprims) && *reinterpret_cast<const unsigned*>(g->indices.data() + (i + 1) * g->indices.stride) == cur + 1;
-        fl[i] = (unsigned char)((hasLeft ? RTC_CURVE_FLAG_NEIGHBOR_LEFT : 0) | (hasRight ? RTC_CURVE_FLAG_NEIGHBOR_RIGHT : 0));
-        hasLeft = hasRight;
-      }
-      d.verts = copy(g->vertices.data(), curveVertBytes, true, "curve vertices");
+      d.verts = copy(g->vertices, curveVertBytes, true, "curve vertices");
       s->residentCurves[g].verts = d.verts;
-      d.idx = copy(g->indices.data(), curveIdxBytes, false, "curve indices");
-      d.flags = copy(fl.data(), nprims, false, "curve flags");
-      cuda_check(cudaStreamSynchronize(0), "upload curve flags");   // `fl` is a stack vector
+      d.idx = copy(g->indices, curveIdxBytes, false, "curve indices");
+      const uint8_t* app = g->flags.buf ? copy(g->flags, (nprims - 1) * g->flags.stride + 1, false, "curve flags") : nullptr;
+      uint8_t* fl = alloc(nprims, false, "curve neighbour flags");
+      cuda_check((cudaError_t)rtk::linear_curve_flags(d.idx, d.istride, app, g->flags.stride, (uint32_t)nprims, fl, 0), "curve flags launch");
+      d.flags = fl;
       d.ntris = (uint32_t)nprims;
       return true;
     }
@@ -458,11 +464,11 @@ struct CommitUpload {
       d.tess = (uint32_t)g->tessellationRate;
       const size_t segs = rtk::prims_per_curve(d);
       if (nprims * segs > 0x7FFFFFFFull || nverts > 0xFFFFFFFFull) fail(RTC_ERROR_INVALID_OPERATION, "curve geometry too large");
-      d.verts = copy(g->vertices.data(), curveVertBytes, true, "curve vertices");
+      d.verts = copy(g->vertices, curveVertBytes, true, "curve vertices");
       s->residentCurves[g].verts = d.verts;
-      d.idx = copy(g->indices.data(), curveIdxBytes, false, "curve indices");
+      d.idx = copy(g->indices, curveIdxBytes, false, "curve indices");
       if (hermite) {
-        d.tangents = copy(g->tangents.data(), nverts ? (nverts - 1) * g->tangents.stride + 16 : 16, true, "curve tangents");
+        d.tangents = copy(g->tangents, nverts ? (nverts - 1) * g->tangents.stride + 16 : 16, true, "curve tangents");
         s->residentCurves[g].tangents = d.tangents;
         d.tstride = g->tangents.stride; d.hermite = 1;
       }
@@ -477,8 +483,8 @@ struct CommitUpload {
     const bool quad = g->type == RTC_GEOMETRY_TYPE_QUAD;
     const size_t ntris = quad ? 2 * nprims : nprims;   // a quad contributes its two halves (quad_intersector_moeller.h:190-200)
     if (ntris > 0x7FFFFFFFull || nverts > 0xFFFFFFFFull) fail(RTC_ERROR_INVALID_OPERATION, "mesh too large");
-    d.verts = copy(g->vertices.data(), nverts ? (nverts - 1) * g->vertices.stride + 12 : 0, false, "vertices");
-    d.idx = copy(g->indices.data(), (nprims - 1) * g->indices.stride + (quad ? 16 : 12), false, "indices");
+    d.verts = copy(g->vertices, nverts ? (nverts - 1) * g->vertices.stride + 12 : 0, false, "vertices");
+    d.idx = copy(g->indices, (nprims - 1) * g->indices.stride + (quad ? 16 : 12), false, "indices");
     d.ntris = (uint32_t)ntris; d.is_quad = quad ? 1 : 0;
     return true;
   }
@@ -1280,6 +1286,8 @@ static void interpolate1(GeometryImpl* g, const RTCInterpolateArguments* a) {
   const BufferView* bv = interp_buffer(g, a->bufferType, a->bufferSlot);
   if (!bv || !g->indices.buf || (kind == rtk::INTERP_HERMITE && !g->tangents.buf)) fail(RTC_ERROR_INVALID_ARGUMENT, "invalid buffer");
   if (a->primID >= g->indices.count) fail(RTC_ERROR_INVALID_ARGUMENT, "invalid primitive ID");
+  if (bv->on_device() || g->indices.on_device() || (kind == rtk::INTERP_HERMITE && g->tangents.on_device()))
+    fail(RTC_ERROR_INVALID_OPERATION, "buffer is in device memory: interpolate with rtcb200InterpolateHits* or rtcb200Interpolate1");
   // dPdv travels with dPdu and the second derivatives with ddPdudu, as in the reference; a curve writes no v-derivative
   const bool curve = rtk::interp_curve(kind);
   float* const out[6] = {a->P, a->dPdu, a->dPdu && !curve ? a->dPdv : nullptr, a->ddPdudu, a->ddPdudu && !curve ? a->ddPdvdv : nullptr,
@@ -1323,15 +1331,17 @@ void rtcInterpolateN(const RTCInterpolateNArguments* a) {
 
 // ---- batched interpolation of hits (rtcb200InterpolateHits*): the scene's interpolation table and its device buffers ----------------
 // Builds the entries of one (buffer type, slot) on `st`: one per geomID of `s`, then one block per instanced scene.  Device copies are
-// shared between entries that read the same host bytes; curve vertex and tangent buffers reuse the copies the commit keeps.
+// shared between entries that read the same bytes -- host memory, or the caller's device memory copied device-to-device; curve vertex
+// and tangent buffers reuse the copies the commit keeps.
 static size_t format_bytes(RTCFormat f);
 struct InterpTableBuild {
   SceneImpl* s;
   SceneImpl::InterpTable& t;
   cudaStream_t st;
-  std::map<std::pair<const char*, size_t>, const uint8_t*> copies;   // (host address, bytes) -> device copy
+  std::map<std::pair<const char*, size_t>, const uint8_t*> copies;   // (address, bytes) -> device copy
 
-  const uint8_t* upload(const char* src, size_t bytes) {
+  const uint8_t* upload(const BufferView& v, size_t bytes) {
+    const char* src = v.data();
     if (!src || bytes == 0) return nullptr;
     const std::pair<const char*, size_t> key(src, bytes);
     auto it = copies.find(key);
@@ -1339,7 +1349,7 @@ struct InterpTableBuild {
     void* p = nullptr;
     cuda_check(cudaMallocAsync(&p, bytes, st), "cudaMallocAsync(interpolation buffer)");
     t.buffers.push_back(p);
-    cuda_check(cudaMemcpyAsync(p, src, bytes, cudaMemcpyHostToDevice, st), "upload interpolation buffer");
+    cuda_check(cudaMemcpyAsync(p, src, bytes, v.copy_kind(), st), "upload interpolation buffer");
     return copies[key] = static_cast<const uint8_t*>(p);
   }
   static size_t span(const BufferView& b) { return b.count ? (b.count - 1) * b.stride + format_bytes(b.format) : 0; }
@@ -1352,14 +1362,14 @@ struct InterpTableBuild {
     if (kind == rtk::INTERP_NONE || !bv || !g->indices.buf || (kind == rtk::INTERP_HERMITE && !g->tangents.buf)) return e;
     e.kind = kind; e.basis = prim_type(g->type).basis;
     e.nprims = (uint32_t)g->indices.count; e.istride = g->indices.stride;
-    e.idx = upload(g->indices.data(), g->indices.count ? (g->indices.count - 1) * g->indices.stride + 4 * rtk::interp_index_count(kind) : 0);
+    e.idx = upload(g->indices, g->indices.count ? (g->indices.count - 1) * g->indices.stride + 4 * rtk::interp_index_count(kind) : 0);
     auto res = s->residentCurves.find(g);
     const bool resident = t.type == RTC_BUFFER_TYPE_VERTEX && res != s->residentCurves.end();
     e.nelems = bv->count; e.dstride = bv->stride;
-    e.data = resident && res->second.verts ? res->second.verts : upload(bv->data(), span(*bv));
+    e.data = resident && res->second.verts ? res->second.verts : upload(*bv, span(*bv));
     if (kind == rtk::INTERP_HERMITE) {
       e.ntang = g->tangents.count; e.tstride = g->tangents.stride;
-      e.tang = resident && res->second.tangents ? res->second.tangents : upload(g->tangents.data(), span(g->tangents));
+      e.tang = resident && res->second.tangents ? res->second.tangents : upload(g->tangents, span(g->tangents));
     }
     return e;
   }
@@ -1534,6 +1544,26 @@ void rtcSetSharedGeometryBuffer(RTCGeometry g, enum RTCBufferType type, unsigned
   b->release();
   GEOM_END
 }
+// The same view of memory on the library's GPU: the buffer is marked as device memory and set_buffer checks it as any other; the
+// commit and the interpolation tables copy it device-to-device (BufferView::copy_kind).
+void rtcb200SetSharedGeometryBufferDevice(RTCGeometry g, enum RTCBufferType type, unsigned int slot, enum RTCFormat format, const void* d_ptr, size_t off,
+                                          size_t stride, size_t num) {
+  GEOM_BEGIN(g)
+  if (num > 0 && !d_ptr) fail(RTC_ERROR_INVALID_ARGUMENT, "device pointer is NULL");
+  if (d_ptr) {
+    cudaPointerAttributes at{};
+    const cudaError_t e = cudaPointerGetAttributes(&at, d_ptr);
+    if (e != cudaSuccess) cudaGetLastError();   // not a pointer CUDA knows: host memory
+    const bool ok = e == cudaSuccess && (at.type == cudaMemoryTypeManaged || (at.type == cudaMemoryTypeDevice && at.device == G(g)->dev->gpu));
+    if (!ok) fail(RTC_ERROR_INVALID_ARGUMENT, "pointer is not device or managed memory on the device's GPU");
+  }
+  BufferImpl* b = new BufferImpl(G(g)->dev, off + (num ? (num - 1) * stride + format_bytes(format) : 0), const_cast<void*>(d_ptr ? d_ptr : (const void*)g));
+  b->device = true;
+  if (!d_ptr) b->ptr = nullptr;   // an empty view: no address, so the getters return NULL and nothing is copied from it
+  try { set_buffer(G(g), type, slot, format, b, off, stride, num); } catch (...) { b->release(); throw; }
+  b->release();
+  GEOM_END
+}
 void* rtcSetNewGeometryBuffer(RTCGeometry g, enum RTCBufferType type, unsigned int slot, enum RTCFormat format, size_t stride, size_t num) {
   GEOM_BEGIN(g)
   size_t bytes = num * stride;
@@ -1546,16 +1576,29 @@ void* rtcSetNewGeometryBuffer(RTCGeometry g, enum RTCBufferType type, unsigned i
   GEOM_END
   return nullptr;
 }
+// the view rtcGetGeometryBufferData[Device] reads
+static const BufferView& geometry_buffer(GeometryImpl* g, RTCBufferType type, unsigned slot) {
+  const BufferView* v = nullptr;
+  if (type == RTC_BUFFER_TYPE_INDEX) { if (slot != 0) fail(RTC_ERROR_INVALID_ARGUMENT, "invalid buffer slot"); v = &g->indices; }
+  else if (type == RTC_BUFFER_TYPE_VERTEX) { if (slot != 0) fail(RTC_ERROR_INVALID_ARGUMENT, "invalid buffer slot"); v = &g->vertices; }
+  else if (type == RTC_BUFFER_TYPE_VERTEX_ATTRIBUTE) { if (slot >= g->attribs.size()) fail(RTC_ERROR_INVALID_ARGUMENT, "invalid buffer slot"); v = &g->attribs[slot]; }
+  else if (type == RTC_BUFFER_TYPE_FLAGS && is_linear_curve(g->type)) { if (slot != 0) fail(RTC_ERROR_INVALID_ARGUMENT, "invalid buffer slot"); v = &g->flags; }
+  else if ((type == RTC_BUFFER_TYPE_TANGENT && is_hermite(g->type)) || (type == RTC_BUFFER_TYPE_NORMAL && g->type == RTC_GEOMETRY_TYPE_ORIENTED_DISC_POINT)) { if (slot != 0) fail(RTC_ERROR_INVALID_ARGUMENT, "invalid buffer slot"); v = &g->tangents; }
+  else fail(RTC_ERROR_INVALID_ARGUMENT, "unknown buffer type");
+  return *v;
+}
 void* rtcGetGeometryBufferData(RTCGeometry g, enum RTCBufferType type, unsigned int slot) {
   GEOM_BEGIN(g)
-  const BufferView* v = nullptr;
-  if (type == RTC_BUFFER_TYPE_INDEX) { if (slot != 0) fail(RTC_ERROR_INVALID_ARGUMENT, "invalid buffer slot"); v = &G(g)->indices; }
-  else if (type == RTC_BUFFER_TYPE_VERTEX) { if (slot != 0) fail(RTC_ERROR_INVALID_ARGUMENT, "invalid buffer slot"); v = &G(g)->vertices; }
-  else if (type == RTC_BUFFER_TYPE_VERTEX_ATTRIBUTE) { if (slot >= G(g)->attribs.size()) fail(RTC_ERROR_INVALID_ARGUMENT, "invalid buffer slot"); v = &G(g)->attribs[slot]; }
-  else if (type == RTC_BUFFER_TYPE_FLAGS && is_linear_curve(G(g)->type)) { if (slot != 0) fail(RTC_ERROR_INVALID_ARGUMENT, "invalid buffer slot"); v = &G(g)->flags; }
-  else if ((type == RTC_BUFFER_TYPE_TANGENT && is_hermite(G(g)->type)) || (type == RTC_BUFFER_TYPE_NORMAL && G(g)->type == RTC_GEOMETRY_TYPE_ORIENTED_DISC_POINT)) { if (slot != 0) fail(RTC_ERROR_INVALID_ARGUMENT, "invalid buffer slot"); v = &G(g)->tangents; }
-  else fail(RTC_ERROR_INVALID_ARGUMENT, "unknown buffer type");
-  return const_cast<char*>(v->data());
+  const BufferView& v = geometry_buffer(G(g), type, slot);
+  if (v.on_device()) fail(RTC_ERROR_INVALID_OPERATION, "buffer is in device memory: it has no host address (rtcGetGeometryBufferDataDevice)");
+  return const_cast<char*>(v.data());
+  GEOM_END
+  return nullptr;
+}
+// a host buffer's host address (its host copy is the source, as for the *HostDevice buffers); a device buffer's device address
+void* rtcGetGeometryBufferDataDevice(RTCGeometry g, enum RTCBufferType type, unsigned int slot) {
+  GEOM_BEGIN(g)
+  return const_cast<char*>(geometry_buffer(G(g), type, slot).data());
   GEOM_END
   return nullptr;
 }
@@ -2065,7 +2108,6 @@ void rtcGetGeometryTransformFromTraversable(RTCTraversable t, unsigned int id, f
 }
 
 // ---- entry points of the reference that are thin variants of supported ones -----------------------------------------
-void* rtcGetGeometryBufferDataDevice(RTCGeometry g, enum RTCBufferType type, unsigned int slot) { return rtcGetGeometryBufferData(g, type, slot); }
 void rtcSetSharedGeometryBufferHostDevice(RTCGeometry g, enum RTCBufferType type, unsigned int slot, enum RTCFormat format, const void* ptr,
                                           const void* /*dptr*/, size_t off, size_t stride, size_t num) {
   rtcSetSharedGeometryBuffer(g, type, slot, format, ptr, off, stride, num);   // buffers are uploaded at commit; the host copy is the source

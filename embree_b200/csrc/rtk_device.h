@@ -136,6 +136,10 @@ int build_scene(SceneGPU& s, const GeomDesc* geoms, int ngeoms, BuilderKind kind
 // Refit the committed BVH to moved vertices (same meshes, same primitive counts, no instances); s.builder becomes 2.
 int refit_scene(SceneGPU& s, const GeomDesc* geoms, int ngeoms, cudaStream_t stream, char* errmsg);
 void free_scene(SceneGPU& s);
+// The neighbour-flag byte of each of the `n` segments of a linear curve geometry into `out` (device): `app` & 3 (one byte per
+// segment, stride `fstride`) when the application set a flags buffer, otherwise derived from the index buffer `idx` (stride
+// `istride`).  All pointers are device copies; enqueued on `stream`.  Returns a CUDA error code.
+int linear_curve_flags(const uint8_t* idx, uint64_t istride, const uint8_t* app, uint64_t fstride, uint32_t n, uint8_t* out, cudaStream_t stream);
 
 struct TraceParams {
   const Node8* nodes;

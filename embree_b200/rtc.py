@@ -288,6 +288,7 @@ class RTCLib:
         "rtcSetSharedGeometryBuffer": (None, [C.c_void_p, C.c_int, C.c_uint, C.c_int, C.c_void_p, C.c_size_t, C.c_size_t, C.c_size_t]),
         "rtcSetNewGeometryBuffer": (C.c_void_p, [C.c_void_p, C.c_int, C.c_uint, C.c_int, C.c_size_t, C.c_size_t]),
         "rtcGetGeometryBufferData": (C.c_void_p, [C.c_void_p, C.c_int, C.c_uint]),
+        "rtcGetGeometryBufferDataDevice": (C.c_void_p, [C.c_void_p, C.c_int, C.c_uint]),
         "rtcUpdateGeometryBuffer": (None, [C.c_void_p, C.c_int, C.c_uint]),
         "rtcSetGeometryTessellationRate": (None, [C.c_void_p, C.c_float]),
         "rtcInterpolate": (None, [C.c_void_p]),
@@ -351,6 +352,7 @@ class RTCLib:
         "rtcb200InterpolateHitsDevice": (None, [C.c_void_p, C.c_void_p, C.c_void_p]),
         "rtcb200GetSceneDeviceTraversable": (None, [C.c_void_p, C.c_void_p]),
         "rtcb200GetSceneDeviceInterpolator": (None, [C.c_void_p, C.c_int, C.c_uint, C.c_void_p]),
+        "rtcb200SetSharedGeometryBufferDevice": (None, [C.c_void_p, C.c_int, C.c_uint, C.c_int, C.c_void_p, C.c_size_t, C.c_size_t, C.c_size_t]),
     }
 
     def __init__(self, path):
@@ -358,6 +360,7 @@ class RTCLib:
             raise FileNotFoundError(f"rtc library not found: {path}")
         self.path = path
         self.dll = C.CDLL(path, mode=C.RTLD_LOCAL)
+        self._device_buffers = {}   # (geometry, buffer type, slot) -> the tensor set_device_buffer attached there
         for name, (res, args) in self._SIGS.items():
             fn = getattr(self.dll, name)
             fn.restype, fn.argtypes = res, args
@@ -519,6 +522,28 @@ class RTCLib:
             gid = geom_id
         self.rtcReleaseGeometry(g)
         return gid
+
+    def set_device_buffer(self, geometry, buffer_type, slot, fmt, tensor, byte_offset=0, byte_stride=None, count=None):
+        """rtcb200SetSharedGeometryBufferDevice with a CUDA torch.Tensor's memory (tensor.data_ptr() + byte_offset).  byte_stride defaults
+        to the bytes of one row of `tensor` (dimension 0), count to its rows.  The tensor is kept referenced here until another tensor is
+        set at the same (geometry, buffer type, slot) or release_device_buffers(geometry) is called, so the memory stays valid while the
+        view is attached.  The commit copies the memory for the build and the trace; the first batched interpolation after a commit
+        copies what it reads, so a scene that will be interpolated needs the tensor unchanged until then.  A refused call (an error
+        recorded on the device) keeps nothing, and leaves the tensor attached before it referenced."""
+        if byte_stride is None:
+            byte_stride = tensor.stride(0) * tensor.element_size() if tensor.dim() > 1 else tensor.element_size()
+        if count is None:
+            count = tensor.shape[0]
+        self.rtcb200SetSharedGeometryBufferDevice(geometry, buffer_type, slot, fmt, C.c_void_p(tensor.data_ptr()), byte_offset, byte_stride, count)
+        # the library records a refusal on the device instead of raising: keep the tensor only when the view now points into it
+        if (self.rtcGetGeometryBufferDataDevice(geometry, buffer_type, slot) or 0) == tensor.data_ptr() + byte_offset:
+            self._device_buffers[(geometry, buffer_type, slot)] = tensor
+
+    def release_device_buffers(self, geometry):
+        """Drops the tensors set_device_buffer keeps for `geometry`: call it once no scene will commit or interpolate the geometry
+        again (a geometry released by the caller but still attached to a scene is copied again by that scene's commits)."""
+        for k in [k for k in self._device_buffers if k[0] == geometry]:
+            del self._device_buffers[k]
 
     def args(self, coherent=False, filter=None, invoke_argument_filter=False, context=None):
         """RTCIntersectArguments / RTCOccludedArguments (same layout).  `filter`: a FILTER_FUNCTION instance (keep it

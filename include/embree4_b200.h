@@ -441,7 +441,8 @@ RTCB200_API double rtcb200GetLastTraceMs(RTCScene scene);
  *    ddPdvdv and ddPdudv not all requested or all omitted (the rtcInterpolateN pairings), a NULL `hits` with M > 0, and a requested
  *    buffer whose format holds fewer than valueCount floats in a geometry that has it.
  *  - Which buffer contents are read: the first call after a commit of the scene (or of an instanced scene, which the scene's own
- *    re-commit follows) uploads the index and data buffers it needs, as their host contents are at that moment, and keeps the
+ *    re-commit follows) copies the index and data buffers it needs, as their contents are at that moment (host memory, or device
+ *    memory of rtcb200SetSharedGeometryBufferDevice), and keeps the
  *    copies until the next commit; curve vertex buffers reuse the copy the commit keeps for the trace kernel.  So an edit to a
  *    buffer is seen after rtcUpdateGeometryBuffer + rtcCommitScene, the rule vertices follow -- unlike rtcInterpolate, which reads
  *    the host buffer as it is.  A commit itself uploads and keeps nothing for interpolation: the first call pays the upload.
@@ -511,8 +512,8 @@ struct RTCB200DeviceGeometryHeader {
 /* Interpolating vertex data from the caller's own CUDA kernels: rtcb200Interpolate1 (embree4_b200_device.cuh) runs, for one hit,
  * the body rtcb200InterpolateHitsDevice runs for every hit of a batch, with the same results bit for bit.
  *  - rtcb200GetSceneDeviceInterpolator fills `out` with the scene's interpolation table for (type, slot): the very table the
- *    batched calls use, built by the first request after a commit -- batched or this getter -- and shared by both.  It uploads
- *    the buffers as their host contents are at that moment (the batched calls' rule).  The build runs on a stream of the calling
+ *    batched calls use, built by the first request after a commit -- batched or this getter -- and shared by both.  It copies
+ *    the buffers as their contents (host or device memory) are at that moment (the batched calls' rule).  The build runs on a stream of the calling
  *    thread's own and is complete when the getter returns.
  *  - Refused, with RTC_ERROR_INVALID_OPERATION recorded, `*out` zeroed and nothing launched: an uncommitted or modified scene, and a
  *    buffer type other than RTC_BUFFER_TYPE_VERTEX (slot 0) or RTC_BUFFER_TYPE_VERTEX_ATTRIBUTE.
@@ -536,6 +537,28 @@ struct RTCB200DeviceInterpolateArguments {
 };
 RTCB200_API void rtcb200GetSceneDeviceInterpolator(RTCScene scene, enum RTCBufferType type, unsigned int slot,
                                                    struct RTCB200DeviceInterpolator* out);
+
+/* Geometry buffers in GPU memory: rtcSetSharedGeometryBuffer with `d_ptr` in device memory (cudaMalloc, a caching allocator's
+ * block, or managed memory) on the library's GPU, for vertices made by the caller's own kernels (skinning, simulation, a tensor).
+ *  - Every buffer type and format rtcSetSharedGeometryBuffer takes, with the same checks and error codes.  Refused with
+ *    RTC_ERROR_INVALID_ARGUMENT and nothing attached: `d_ptr` in host memory (pageable or pinned), in another GPU's memory, or
+ *    NULL with itemCount > 0.
+ *  - rtcCommitScene copies the buffer device-to-device on the library's own stream and builds from that copy, as it uploads a host
+ *    buffer: the caller's writes must be complete before rtcCommitScene (synchronise the stream that wrote them).
+ *    rtcUpdateGeometryBuffer and rtcCommitGeometry mark edits as for host buffers.
+ *  - What must stay valid: as for a host shared buffer, the memory belongs to the geometry while it is attached.  The BVH and the
+ *    records the queries read never refer to it after rtcCommitScene returns, so a caller that only traces may overwrite it then.
+ *    Interpolation does read it: the first rtcb200InterpolateHits* or rtcb200GetSceneDeviceInterpolator request after a commit
+ *    copies the index, vertex, vertex-attribute and tangent buffers it needs (device-to-device) as they are at that moment.  Keep
+ *    them valid and unchanged from the commit until that request if the scene will be interpolated, and do not free them while a
+ *    scene that may commit the geometry again holds it.
+ *  - rtcGetGeometryBufferDataDevice returns d_ptr + byteOffset; rtcGetGeometryBufferData records RTC_ERROR_INVALID_OPERATION and
+ *    returns NULL (there is no host address).  rtcInterpolate / rtcInterpolateN on a buffer in device memory -- the requested one,
+ *    the index buffer or a Hermite curve's tangents -- record RTC_ERROR_INVALID_OPERATION and write nothing: interpolate such
+ *    geometry with rtcb200InterpolateHits* or rtcb200Interpolate1. */
+RTCB200_API void rtcb200SetSharedGeometryBufferDevice(RTCGeometry geometry, enum RTCBufferType type, unsigned int slot,
+                                                      enum RTCFormat format, const void* d_ptr, size_t byteOffset,
+                                                      size_t byteStride, size_t itemCount);
 
 /* =====================================================================================================
  * Section C -- the rest of the reference library's export list (kernels/export.linux.map: every rtc* symbol).
