@@ -24,7 +24,9 @@ __device__ __forceinline__ float rcp_safe_fast(float d) {
 // triangle; the ray is taken into that space with the instance's world2local exactly as the reference does before it
 // traces the instanced scene (xfmPoint / xfmVector, affinespace.h:102-103) -- t is unchanged by the affine map, so the
 // world-space BVH above and the object-space triangle test below share one parametrisation.
-__device__ __forceinline__ void to_object_space(const GeomDesc& d, Ray& r) {
+// `d` is a GeomDesc, or the InstRec of instance traversal (trace.cu, INST), which applies the same map when a ray enters an instance.
+template <typename Xfm>
+__device__ __forceinline__ void to_object_space(const Xfm& d, Ray& r) {
   const float ox = r.ox, oy = r.oy, oz = r.oz, dx = r.dx, dy = r.dy, dz = r.dz;
   r.ox = fma_rn(ox, d.w2l[0], fma_rn(oy, d.w2l[3], fma_rn(oz, d.w2l[6], d.w2l[9])));
   r.oy = fma_rn(ox, d.w2l[1], fma_rn(oy, d.w2l[4], fma_rn(oz, d.w2l[7], d.w2l[10])));

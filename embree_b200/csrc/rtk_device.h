@@ -21,11 +21,12 @@ enum PrimKind : uint32_t {
   PRIM_SPHERE = 5,          // point kinds: point_test's point type is kind - PRIM_SPHERE
   PRIM_DISC = 6,            // ray-facing disc
   PRIM_ORIENTED_DISC = 7,   // disc with a normal (in `tangents`, stride `tstride`)
+  PRIM_INSTANCE = 8,        // instance traversal's top level: one primitive per instance, `verts` = the scene's InstRec table
 };
 // The kernels write `kind >= PRIM_SPHERE` out instead of calling point_record: even inlined, the call changes how the compiler lays
 // out their if-chains over the kinds.
 RT_HD constexpr bool curve_record(uint32_t kind) { return kind >= PRIM_ROUND_LINEAR && kind <= PRIM_ROUND_CUBIC; }
-RT_HD constexpr bool point_record(uint32_t kind) { return kind >= PRIM_SPHERE; }   // PRIM_ORIENTED_DISC is the last kind
+RT_HD constexpr bool point_record(uint32_t kind) { return kind >= PRIM_SPHERE && kind <= PRIM_ORIENTED_DISC; }
 
 // one enabled triangle mesh, buffers already resident on the device (raw bytes, caller's stride honoured:
 // kernels/common/buffer.h BufferView semantics)
@@ -58,6 +59,20 @@ struct GeomDesc {
   float xfm[12] = {1, 0, 0, 0, 1, 0, 0, 0, 1, 0, 0, 0};
   float w2l[12] = {1, 0, 0, 0, 1, 0, 0, 0, 1, 0, 0, 0};
 };
+
+// Instance traversal (commit path for scenes whose flattened copy would be large): the top level holds one record per instance, and a
+// ray that reaches it continues, in object space, through one BVH of the instanced scene laid out in the same node / record arrays.
+// One InstRec per instance.  `lo`, `hi`: bounds of the instanced scene's BVH (object space), boxed through `xfm` by the builder.
+struct InstRec {
+  float w2l[12];          // world2local, the columns to_object_space reads
+  uint32_t instID, mask;  // geomID of the instance in its scene, instance mask
+  uint32_t child_root;    // node index of the instanced scene's root in the scene's node array
+  uint32_t pad;
+  float xfm[12];          // local2world
+  float lo[3], hi[3];
+};
+// b.w of an instance record (instance index in a.w, instance mask in c.w); every other record holds a descriptor index there
+constexpr uint32_t kInstRecord = 0xFFFFFFFEu;
 
 // BVH primitives per curve of a cubic curve geometry: the sweep's first-level sub-segments (round) or the ribbon's tessellation
 // segments (flat).  Primitive `curve * prims_per_curve + segment` is that segment of that curve.
@@ -121,7 +136,28 @@ struct SceneGPU {
   std::vector<const void*> sub_id;      // which sub-BVH object occupies each slot (a different one there is copied even if the counts match)
   uint32_t top_cap = 0;                 // nodes reserved at the start of the array for the top level
   bool is_sub = false;                  // a per-mesh BVH of a two-level scene: never traced on its own (no stat counters)
+  InstRec* d_insts = nullptr;           // instance traversal: the instance table (NULL on every other path)
+  uint32_t num_insts = 0;
+  uint32_t top_tri_cap = 0;             // instance traversal: records reserved after the instanced scenes for the top level
 };
+
+// ---- instance traversal (assemble_instanced).  Node 0 holds a copy of the top level's root; then every instanced scene's BVH, in the
+// order given, then the top level.  Records: the instanced scenes', then the top level's.  `node_off[i]` is also where scene i's root
+// lands, which the InstRecs need before the top level is built.
+struct InstanceLayout { std::vector<uint32_t> node_off, tri_off; uint32_t kid_nodes = 1, kid_tris = 0; };
+inline InstanceLayout instance_layout(SceneGPU* const* kids, int nkids) {
+  InstanceLayout L;
+  for (int i = 0; i < nkids; ++i) {
+    L.node_off.push_back(L.kid_nodes); L.tri_off.push_back(L.kid_tris);
+    if (kids[i]->root_valid) { L.kid_nodes += kids[i]->num_nodes; L.kid_tris += kids[i]->num_tris; }
+  }
+  return L;
+}
+// Lays the instanced scenes' BVHs `kids` (records through descriptors, relocated by kid_desc_off[i]) and the top level `top` (own
+// primitives and one instance record per instance, descriptors relocated by top_desc_off) out in s's arrays.  kids_same: the same
+// BVHs as at the last call, unchanged -- they are then left in place when the top level fits.
+int assemble_instanced(SceneGPU& s, const SceneGPU& top, SceneGPU* const* kids, const uint32_t* kid_desc_off, int nkids, uint32_t top_desc_off,
+                       bool kids_same, cudaStream_t stream, char* errmsg);
 
 // ---- two-level scenes (kernels/bvh/bvh_builder_twolevel.cpp:35-240: dynamic scenes keep one BVH per mesh and rebuild only what
 // changed).  Every mesh is built on its own (build_scene / refit_scene on a one-mesh SceneGPU, kept by the host shim); assemble_scene
@@ -164,6 +200,7 @@ struct TraceParams {
   const uint32_t* excl_off = nullptr;
   const uint32_t* excl_idx = nullptr;
   uint32_t* win = nullptr;
+  const InstRec* insts = nullptr;   // instance traversal: the instance table the top level's instance records index
 };
 // occluded: 0 = closest hit (rtcIntersect*), 1 = any hit (rtcOccluded*); K in {1,4,8,16}
 int launch_trace(const TraceParams& p, int occluded, int K, cudaStream_t stream);
@@ -199,6 +236,10 @@ struct Tuning {
   int tri_spread = 1;        // warp-wide triangle redistribution in the trace kernel (trace.cu SPREAD; closest-hit triangle scenes)
   int tri_spread_occluded = 1;   // the same redistribution in the any-hit kernels (a hit ends the owner's ray)
   int sah_small = 4;         // SAH builder: segments of <= this many primitives are split in the middle (no binning)
+  // a scene with instances and no filter callbacks commits through instance traversal when flattening it would make more than this
+  // many records (sum over the instances of the instanced scene's records).  The default leaves every scene whose flattened copy can
+  // be built flattened (rtcore_shim.cpp choose_instance_traversal): only flattened scenes serve device-side queries and filters.
+  int instance_flatten_max = 2147483647;
 };
 Tuning& tuning();
 

@@ -148,7 +148,14 @@ __device__ __forceinline__ void tma_prefetch_l2(const void* src, uint32_t bytes)
 // trace_filtered).  Every ray carries a list of record indices that a callback has already rejected
 // (p.excl_idx[p.excl_off[i] .. p.excl_off[i+1])); those records are skipped, and the winning record's index goes to p.win[i]
 // so that the host can extend the list when the callback rejects this hit as well.
-template <int K, bool OCCLUDED, bool STATS, bool ROBUST, int GENERAL, int GATHER = 0, bool SPREAD = false, bool FILTER = false>
+//
+// INST (instance traversal, GENERAL >= 1): the top level's instance records (b.w == kInstRecord) are entered instead of tested.  The
+// lane checks the instance mask, pushes what is left of its node group and of its leaf group, then an exit marker (y == 0), takes
+// the ray into object space with the instance's w2l (to_object_space: the records see the ray flattening gives them), recomputes
+// 1/dir and the octant, and continues at the instanced scene's root.  Popping the marker reloads the world ray from the ray buffer;
+// t is shared by both spaces, so the hit distance carries over.  The entries under the marker were pushed in world space and are
+// decoded with the world octant again.  A leaf group on the stack has no pending-child bits (y & 0xFF000000 == 0, y != 0).
+template <int K, bool OCCLUDED, bool STATS, bool ROBUST, int GENERAL, int GATHER = 0, bool SPREAD = false, bool FILTER = false, bool INST = false>
 __global__ void __launch_bounds__(TRACE_THREADS, RTK_MIN_BLOCKS) trace_kernel(const TraceParams p) {
   const bool USE_TMA = p.use_prefetch != 0;
   using IO = RayIO<K, OCCLUDED>;
@@ -174,12 +181,15 @@ __global__ void __launch_bounds__(TRACE_THREADS, RTK_MIN_BLOCKS) trace_kernel(co
   // other values inside the node step otherwise.
   // GENERAL == 2 (curve scenes): 9-11 the normal of a curve hit -- the round cubic test is an iteration whose result depends on
   // the tfar it was started with, so the normal is kept from the winning test instead of re-running the test at write-back
-  __shared__ uint32_t s_lane[GENERAL == 2 ? 12 : 9][TRACE_THREADS];   // 0 u, 1 v, 2 winning record, 3 ray index, 4-6 ray direction, 7 ray mask, 8 the ray's own tfar
+  // INST: two more, the instance the lane is in (kInvalidID: none) and that of the winning record
+  __shared__ uint32_t s_lane[(GENERAL == 2 ? 12 : 9) + (INST ? 2 : 0)][TRACE_THREADS];   // 0 u, 1 v, 2 winning record, 3 ray index, 4-6 ray direction, 7 ray mask, 8 the ray's own tfar
 #define hit_u (reinterpret_cast<float*>(s_lane[0])[threadIdx.x])
 #define hit_v (reinterpret_cast<float*>(s_lane[1])[threadIdx.x])
 #define hit_tri (s_lane[2][threadIdx.x])
 #define ray_index (s_lane[3][threadIdx.x])
 #define CURVE_NG(k) (s_lane[GENERAL == 2 ? 9 + (k) : 0][threadIdx.x])
+#define CUR_INST (s_lane[INST ? (GENERAL == 2 ? 12 : 9) : 0][threadIdx.x])
+#define HIT_INST (s_lane[INST ? (GENERAL == 2 ? 13 : 10) : 0][threadIdx.x])
   // The ray's direction, mask and original tfar are only needed by triangle / curve tests: the node step works with
   // org, 1/dir, tnear and the current hit distance.  They are parked in shared memory too (read by the SPREAD workers by
   // owner index -- instead of five shuffles -- and by the non-SPREAD test of the lane itself).
@@ -251,7 +261,15 @@ __global__ void __launch_bounds__(TRACE_THREADS, RTK_MIN_BLOCKS) trace_kernel(co
       else {   // Ng and the ids come from the winning record, re-read here
         Hit hit;
         uint32_t instID = p.instID, instPrimID = p.instPrimID;
-        record_write_back<ROBUST, GENERAL>(tris, p.descs, hit_tri, full_ray, curve_normal, hit_u, hit_v, hit, instID, instPrimID);
+        if constexpr (INST) {
+          // a record hit inside an instance reports the instance's ids, and ROBUST's Ng takes the object-space origin
+          const uint32_t hi = HIT_INST;
+          auto hit_ray = [&]() -> Ray { Ray q = full_ray(); if (hi != kInvalidID) to_object_space(p.insts[hi], q); return q; };
+          record_write_back<ROBUST, GENERAL>(tris, p.descs, hit_tri, hit_ray, curve_normal, hit_u, hit_v, hit, instID, instPrimID);
+          if (hi != kInvalidID) { instID = p.insts[hi].instID; instPrimID = 0u; }   // instance_id_stack::push(context, instID, 0)
+        } else {
+          record_write_back<ROBUST, GENERAL>(tris, p.descs, hit_tri, full_ray, curve_normal, hit_u, hit_v, hit, instID, instPrimID);
+        }
         hit.t = tfar_tri;
         IO::store_hit(p, ray_index, hit, instID, instPrimID);
         cngx = hit.ngx; cngy = hit.ngy; cngz = hit.ngz; cprim = hit.primID; cgeom = hit.geomID;
@@ -285,6 +303,7 @@ __global__ void __launch_bounds__(TRACE_THREADS, RTK_MIN_BLOCKS) trace_kernel(co
       if (OCCLUDED) { ngy = 0; tgy = 0; sp = 0; top_y = 0; }     // any hit terminates the ray
       else {
         tfar_tri = h.t; hit_tri = ti;
+        if constexpr (INST) HIT_INST = CUR_INST;
         if (GENERAL == 2 && h.curve) { CURVE_NG(0) = __float_as_uint(h.ngx); CURVE_NG(1) = __float_as_uint(h.ngy); CURVE_NG(2) = __float_as_uint(h.ngz); }
       }
     });
@@ -357,6 +376,7 @@ __global__ void __launch_bounds__(TRACE_THREADS, RTK_MIN_BLOCKS) trace_kernel(co
               if (STATS) ++st_rays;
               found = false;
               sp = 0; top_y = 0; tgx = 0; tgy = 0;
+              if constexpr (INST) { CUR_INST = kInvalidID; HIT_INST = kInvalidID; }
               // empty scene / already occluded rays terminate at once (bvh_intersector1.cpp:39,128-129); they still
               // pass through DONE so that a gather buffer receives their miss record
               const bool go = p.root_valid && !(OCCLUDED && r.tfar < 0.0f);
@@ -497,7 +517,31 @@ __global__ void __launch_bounds__(TRACE_THREADS, RTK_MIN_BLOCKS) trace_kernel(co
         const uint4* tp = tris + (size_t)ti * 3;
         const uint4 a = __ldg(tp), b = __ldg(tp + 1), c = __ldg(tp + 2);
         if (STATS) ++st_tris;
-        if (RTK_TRI2) {
+        if constexpr (INST) {
+          // an instance record (instance index in a.w, its mask in c.w): enter the instance instead of testing a record.  What is
+          // left of the node and leaf groups goes on the stack, then the exit marker.
+          if (b.w == kInstRecord) {
+            if ((c.w & RAY_MASK(threadIdx.x)) != 0) {   // instance_intersector.cpp:19-22
+              const InstRec& ir = p.insts[a.w];
+              if (top_y) push_entry(top_x, top_y);
+              top_y = 0;
+              if (ngy & 0xFF000000u) push_entry(ngx, ngy);
+              if (tgy) push_entry(tgx, tgy);
+              push_entry(0u, 0u);
+              Ray q = full_ray();
+              to_object_space(ir, q);
+              r.ox = q.ox; r.oy = q.oy; r.oz = q.oz;
+              RAY_DX(threadIdx.x) = q.dx; RAY_DY(threadIdx.x) = q.dy; RAY_DZ(threadIdx.x) = q.dz;
+              idx = rcp_safe_fast(q.dx); idy = rcp_safe_fast(q.dy); idz = rcp_safe_fast(q.dz);
+              oct = (idx < 0.0f ? 1u : 0u) | (idy < 0.0f ? 2u : 0u) | (idz < 0.0f ? 4u : 0u);
+              CUR_INST = a.w;
+              ngx = __ldg(&ir.child_root); ngy = 0x80000000u;   // the instanced scene's root, entered like the scene root at refill
+              tgy = 0;
+            }
+          } else {
+            test_tri(ti, a, b, c);   // one record per step: a second one could be an instance
+          }
+        } else if (RTK_TRI2) {
           // a second pending triangle of the same lane rides along: its record is fetched together with the first
           // (one latency instead of two) and tested after it, against the tfar the first one left -- the sequential order
           const bool two = tgy != 0;
@@ -520,7 +564,23 @@ __global__ void __launch_bounds__(TRACE_THREADS, RTK_MIN_BLOCKS) trace_kernel(co
     // ---- 4. pop or finish
     if (tracing && tgy == 0 && (ngy & 0xFF000000u) == 0) {
       if (top_y) { ngx = top_x; ngy = top_y; top_y = 0; }
-      else if (sp > 0) { const uint2 e = pop_entry(); ngx = e.x; ngy = e.y; }
+      else if (sp > 0) {
+        const uint2 e = pop_entry();
+        ngx = e.x; ngy = e.y;
+        if constexpr (INST) {
+          if ((e.y & 0xFF000000u) == 0) {   // a leaf group, or the exit marker of an instance
+            ngy = 0;
+            if (e.y) { tgx = e.x; tgy = e.y; }
+            else {   // back in world space: the ray from the ray buffer, its reciprocal and octant as the refill set them up
+              IO::load(static_cast<const char*>(p.rays), ray_index, r);
+              RAY_DX(threadIdx.x) = r.dx; RAY_DY(threadIdx.x) = r.dy; RAY_DZ(threadIdx.x) = r.dz;
+              idx = rcp_safe_fast(r.dx); idy = rcp_safe_fast(r.dy); idz = rcp_safe_fast(r.dz);
+              oct = (idx < 0.0f ? 1u : 0u) | (idy < 0.0f ? 2u : 0u) | (idz < 0.0f ? 4u : 0u);
+              CUR_INST = kInvalidID;
+            }
+          }
+        }
+      }
       else state = DONE;
     }
   }
@@ -545,6 +605,8 @@ __global__ void __launch_bounds__(TRACE_THREADS, RTK_MIN_BLOCKS) trace_kernel(co
 #undef hit_tri
 #undef ray_index
 #undef CURVE_NG
+#undef CUR_INST
+#undef HIT_INST
 #undef RAY_DX
 #undef RAY_DY
 #undef RAY_DZ
@@ -594,7 +656,7 @@ static int launch_k(TraceParams p, cudaStream_t st) {
   const int variant = (p.stat ? 4 : 0) | (p.robust ? 2 : 0) | (p.descs ? 1 : 0);
   const int g = general_of(p.descs, p.curves);
   if (p.excl_off) {   // filter-callback passes (rtcore_shim.cpp trace_filtered): K == 1 closest hit, no gather, no statistics
-    if (!(K == 1 && CLOSEST) || !p.excl_idx || !p.win) return (int)cudaErrorInvalidValue;
+    if (!(K == 1 && CLOSEST) || !p.excl_idx || !p.win || p.insts) return (int)cudaErrorInvalidValue;
     constexpr bool FI = (K == 1 && CLOSEST);   // only these instantiations carry the exclusion code
     switch (g * 2 + (p.robust ? 1 : 0)) {
 #define RTK_FILTER(RB, GE) trace_kernel<K, OCCLUDED, false, RB, GE, 0, false, FI><<<blocks, TRACE_THREADS, 0, st>>>(p); break
@@ -605,6 +667,27 @@ static int launch_k(TraceParams p, cudaStream_t st) {
       case 4: RTK_FILTER(false, 2);
       case 5: RTK_FILTER(true, 2);
 #undef RTK_FILTER
+    }
+    count_launch();
+    return (int)cudaGetLastError();
+  }
+  if (p.insts) {   // instance traversal: the INST instantiations, GENERAL 1 or 2
+    const int gmode = (CAN_GATHER && p.compact_out) ? ((g_tuning.gather_mode == 0 || !p.stage) ? 1 : 2) : 0;
+    switch ((variant >> 1) + 4 * gmode + (g == 2 ? 12 : 0)) {
+#define RTK_INST(ST, RB, GE, GA) trace_kernel<K, OCCLUDED, ST, RB, GE, (CAN_GATHER ? GA : 0), false, false, true><<<blocks, TRACE_THREADS, 0, st>>>(p); break
+#define RTK_INST4(GE, GA)                                              \
+      case (GE == 2 ? 12 : 0) + 4 * GA + 0: RTK_INST(false, false, GE, GA); \
+      case (GE == 2 ? 12 : 0) + 4 * GA + 1: RTK_INST(false, true, GE, GA);  \
+      case (GE == 2 ? 12 : 0) + 4 * GA + 2: RTK_INST(true, false, GE, GA);  \
+      case (GE == 2 ? 12 : 0) + 4 * GA + 3: RTK_INST(true, true, GE, GA);
+      RTK_INST4(1, 0)
+      RTK_INST4(1, 1)
+      RTK_INST4(1, 2)
+      RTK_INST4(2, 0)
+      RTK_INST4(2, 1)
+      RTK_INST4(2, 2)
+#undef RTK_INST4
+#undef RTK_INST
     }
     count_launch();
     return (int)cudaGetLastError();
