@@ -838,8 +838,15 @@ static cudaError_t alloc_stat(SceneGPU& s, cudaStream_t st) {
   return e == cudaSuccess ? cudaMemsetAsync(s.d_stat, 0, 3 * sizeof(unsigned long long), st) : e;
 }
 
-// the BVH arrays and what refit_scene keeps (pool memory: goes back to the pool for the next commit)
+// the arrays of `s` are about to change (SceneGPU::content)
+static void renew_content(SceneGPU& s) {
+  static std::atomic<uint64_t> last{0};
+  s.content = ++last;
+}
+
+// the BVH arrays, what refit_scene keeps and the layout of an assembly (pool memory: goes back to the pool for the next commit)
 static void release_arrays(SceneGPU& s, cudaStream_t st) {
+  renew_content(s);
   if (s.nodes) cudaFreeAsync(s.nodes, st);
   if (s.tris) cudaFreeAsync(s.tris, st);
   if (s.d_descs) cudaFreeAsync(s.d_descs, st);
@@ -848,6 +855,7 @@ static void release_arrays(SceneGPU& s, cudaStream_t st) {
   s.nodes = nullptr; s.tris = nullptr; s.d_descs = nullptr; s.tri_src = nullptr; s.d_insts = nullptr; s.levels.clear();
   s.num_insts = 0;
   s.num_nodes = s.num_tris = 0; s.root_valid = 0;
+  s.subs.clear(); s.top_cap = s.top_tri_cap = 0;
 }
 
 void free_scene(SceneGPU& s) {
@@ -858,7 +866,7 @@ void free_scene(SceneGPU& s) {
 
 int build_scene(SceneGPU& s, const GeomDesc* geoms, int ngeoms, BuilderKind kind, cudaStream_t st, char* errmsg) {
   errmsg[0] = 0;
-  release_arrays(s, st);
+  release_arrays(s, st);   // renews s.content
   s.max_depth = 0; s.sah_cost = 0; s.builder = kind;
   for (int a = 0; a < 3; ++a) { s.bounds[a] = s.api_bounds[a] = INFINITY; s.bounds[3 + a] = s.api_bounds[3 + a] = -INFINITY; }
   if (!s.is_sub) CK(alloc_stat(s, st));
@@ -1042,6 +1050,7 @@ int refit_scene(SceneGPU& s, const GeomDesc* geoms, int ngeoms, cudaStream_t st,
   if (!s.root_valid || !s.tri_src || s.levels.size() < 2) { snprintf(errmsg, 256, "refit: scene has no kept topology"); return -1; }
   std::vector<uint32_t> offs;
   if (prim_offsets(geoms, ngeoms, offs) != s.total_prims) { snprintf(errmsg, 256, "refit: primitive count changed"); return -1; }
+  renew_content(s);
   ensure_pool(s.device);
   EventTimer timer;
   CK(timer.start(st));
@@ -1064,7 +1073,7 @@ int refit_scene(SceneGPU& s, const GeomDesc* geoms, int ngeoms, cudaStream_t st,
   CK(cudaStreamSynchronize(st));
   CK(cudaGetLastError());
   for (int a = 0; a < 6; ++a) s.bounds[a] = s.api_bounds[a] = rb[a];
-  s.build_ms = timer.ms(); s.builder = 2;
+  s.build_ms = timer.ms(); s.builder = BUILDER_REFIT;
   return 0;
 }
 
@@ -1105,51 +1114,48 @@ __global__ void __launch_bounds__(256) relocate_nodes(const Node8* __restrict__ 
 }
 
 
-int assemble_scene(SceneGPU& s, SceneGPU* const* subs, int nsubs, const uint8_t* dirty, cudaStream_t st, char* errmsg) {
+int assemble_scene(SceneGPU& s, SceneGPU* const* subs, int nsubs, cudaStream_t st, char* errmsg) {
   errmsg[0] = 0;
+  renew_content(s);
   ensure_pool(s.device);
   CK(alloc_stat(s, st));
   EventTimer timer;
   CK(timer.start(st));
-  // same layout as last time?  (same number of subs, each with unchanged node / record counts)
-  bool same = s.nodes && s.tris && (int)s.sub_nodes.size() == nsubs;
+  const uint32_t top_cap = (uint32_t)(2 * nsubs + 8);
+  uint64_t nn, nt;
+  const std::vector<SubSlot> L = sub_layout(subs, nsubs, top_cap, nn, nt);
+  // same layout as last time?  (every sub in its place, with unchanged node / record counts)
+  bool same = s.nodes && s.tris && s.subs.size() == L.size();
   for (int i = 0; same && i < nsubs; ++i)
-    same = s.sub_nodes[i] == (subs[i]->root_valid ? subs[i]->num_nodes : 0u) && s.sub_tris[i] == (subs[i]->root_valid ? subs[i]->num_tris : 0u);
+    same = s.subs[i].node_off == L[i].node_off && s.subs[i].nodes == L[i].nodes && s.subs[i].tris == L[i].tris;
   if (!same) {
     if (s.nodes) { cudaFreeAsync(s.nodes, st); s.nodes = nullptr; }
     if (s.tris) { cudaFreeAsync(s.tris, st); s.tris = nullptr; }
-    s.sub_node_off.assign(nsubs, 0); s.sub_tri_off.assign(nsubs, 0); s.sub_nodes.assign(nsubs, 0); s.sub_tris.assign(nsubs, 0);
-    s.sub_root.assign(nsubs, Node8{});
-    s.sub_id.assign(nsubs, nullptr);
-    s.top_cap = (uint32_t)(2 * nsubs + 8);
-    uint64_t nn = s.top_cap, nt = 0;
-    for (int i = 0; i < nsubs; ++i) {
-      s.sub_node_off[i] = (uint32_t)nn; s.sub_tri_off[i] = (uint32_t)nt;
-      if (!subs[i]->root_valid) continue;
-      s.sub_nodes[i] = subs[i]->num_nodes; s.sub_tris[i] = subs[i]->num_tris;
-      nn += subs[i]->num_nodes; nt += subs[i]->num_tris;
-    }
+    s.subs = L; s.top_cap = top_cap;
     if (nn >= 0x7FFFFFFFull || nt >= 0x7FFFFFFFull) { snprintf(errmsg, 256, "two-level scene too large"); return -1; }
     CK(cudaMallocAsync(reinterpret_cast<void**>(&s.nodes), std::max<uint64_t>(nn, 1) * sizeof(Node8), st));
     CK(cudaMallocAsync(reinterpret_cast<void**>(&s.tris), std::max<uint64_t>(nt, 1) * sizeof(TriRec), st));
     s.num_nodes = (uint32_t)nn; s.num_tris = (uint32_t)nt;
   }
-  for (int i = 0; i < nsubs; ++i) {
+  for (int i = 0; i < nsubs; ++i) {   // a slot is copied when it holds no copy of its sub-BVH as it is now
     const SceneGPU& b = *subs[i];
-    const bool other = s.sub_id[i] != static_cast<const void*>(subs[i]);   // another mesh took this slot
-    s.sub_id[i] = subs[i];
-    if (!b.root_valid || (same && !dirty[i] && !other)) continue;
-    relocate_nodes<<<(b.num_nodes + 255) / 256, 256, 0, st>>>(b.nodes, b.num_nodes, s.nodes + s.sub_node_off[i], s.sub_node_off[i], s.sub_tri_off[i]);
+    SubSlot& sl = s.subs[i];
+    if (sl.content == b.content) continue;
+    sl.content = b.content;
+    if (!b.root_valid) continue;
+    relocate_nodes<<<(b.num_nodes + 255) / 256, 256, 0, st>>>(b.nodes, b.num_nodes, s.nodes + sl.node_off, sl.node_off, sl.tri_off);
     count_launch();
-    CK(cudaMemcpyAsync(s.tris + s.sub_tri_off[i], b.tris, (size_t)b.num_tris * sizeof(TriRec), cudaMemcpyDeviceToDevice, st));
-    CK(cudaMemcpyAsync(&s.sub_root[i], s.nodes + s.sub_node_off[i], sizeof(Node8), cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(s.tris + sl.tri_off, b.tris, (size_t)b.num_tris * sizeof(TriRec), cudaMemcpyDeviceToDevice, st));
+    CK(cudaMemcpyAsync(&sl.root, s.nodes + sl.node_off, sizeof(Node8), cudaMemcpyDeviceToHost, st));
   }
   CK(cudaStreamSynchronize(st));   // the relocated root nodes are on the host now
   CK(cudaGetLastError());
   // top level on the host: a few hundred meshes at most cost microseconds here
   std::vector<TopItem> items;
+  std::vector<Node8> roots;
   for (int a = 0; a < 3; ++a) { s.bounds[a] = s.api_bounds[a] = INFINITY; s.bounds[3 + a] = s.api_bounds[3 + a] = -INFINITY; }
   for (int i = 0; i < nsubs; ++i) {
+    roots.push_back(s.subs[i].root);
     if (!subs[i]->root_valid) continue;
     TopItem it;
     for (int a = 0; a < 3; ++a) {
@@ -1162,14 +1168,14 @@ int assemble_scene(SceneGPU& s, SceneGPU* const* subs, int nsubs, const uint8_t*
   s.root_valid = items.empty() ? 0u : 1u;
   s.levels.clear();
   if (!items.empty()) {
-    const std::vector<Node8> top = build_top_level(items, s.sub_root);
+    const std::vector<Node8> top = build_top_level(items, roots);
     if (top.size() > s.top_cap) { snprintf(errmsg, 256, "internal: top level needs %zu of %u nodes", top.size(), s.top_cap); return -1; }
     CK(cudaMemcpyAsync(s.nodes, top.data(), top.size() * sizeof(Node8), cudaMemcpyHostToDevice, st));
     s.levels = {0u, s.num_nodes};
   }
   CK(timer.stop(st));
   CK(cudaStreamSynchronize(st));
-  s.build_ms = timer.ms(); s.builder = 3; s.max_depth = 0; s.sah_cost = 0;
+  s.build_ms = timer.ms(); s.builder = BUILDER_TWO_LEVEL; s.max_depth = 0; s.sah_cost = 0;
   return 0;
 }
 
@@ -1186,39 +1192,44 @@ __global__ void __launch_bounds__(256) relocate_records(const TriRec* __restrict
 }
 
 int assemble_instanced(SceneGPU& s, const SceneGPU& top, SceneGPU* const* kids, const uint32_t* kid_desc_off, int nkids, uint32_t top_desc_off,
-                       bool kids_same, cudaStream_t st, char* errmsg) {
+                       cudaStream_t st, char* errmsg) {
   errmsg[0] = 0;
+  renew_content(s);
   CK(alloc_stat(s, st));
   EventTimer timer;
   CK(timer.start(st));
-  const InstanceLayout L = instance_layout(kids, nkids);
+  uint64_t kn, kt;
+  std::vector<SubSlot> L = sub_layout(kids, nkids, 1, kn, kt);
+  const uint32_t kid_nodes = (uint32_t)kn, kid_tris = (uint32_t)kt;
   const uint32_t tn = top.root_valid ? top.num_nodes : 0u, tt = top.root_valid ? top.num_tris : 0u;
-  // the instanced scenes stay where they are while they are the same and the top level fits the room left for it
-  const bool keep = kids_same && s.nodes && s.tris && s.sub_node_off == L.node_off && tn <= s.top_cap && tt <= s.top_tri_cap;
+  // the instanced scenes stay where they are while every slot holds the same BVH and the top level fits the room left for it
+  bool keep = s.nodes && s.tris && s.subs.size() == L.size() && tn <= s.top_cap && tt <= s.top_tri_cap;
+  for (int i = 0; keep && i < nkids; ++i) keep = s.subs[i].content == kids[i]->content;
   if (!keep) {
     if (s.nodes) { cudaFreeAsync(s.nodes, st); s.nodes = nullptr; }
     if (s.tris) { cudaFreeAsync(s.tris, st); s.tris = nullptr; }
     s.top_cap = tn + tn / 2 + 16; s.top_tri_cap = tt + tt / 2 + 16;   // room for a top level that grows a little between commits
-    const uint64_t nn = (uint64_t)L.kid_nodes + s.top_cap, nt = (uint64_t)L.kid_tris + s.top_tri_cap;
+    const uint64_t nn = kn + s.top_cap, nt = kt + s.top_tri_cap;
     if (nn >= 0x7FFFFFFFull || nt >= 0x7FFFFFFFull) { snprintf(errmsg, 256, "instanced scene too large"); return -1; }
     CK(cudaMallocAsync(reinterpret_cast<void**>(&s.nodes), nn * sizeof(Node8), st));
     CK(cudaMallocAsync(reinterpret_cast<void**>(&s.tris), nt * sizeof(TriRec), st));
     for (int i = 0; i < nkids; ++i) {
       const SceneGPU& b = *kids[i];
+      L[i].content = b.content;
       if (!b.root_valid) continue;
-      relocate_nodes<<<(b.num_nodes + 255) / 256, 256, 0, st>>>(b.nodes, b.num_nodes, s.nodes + L.node_off[i], L.node_off[i], L.tri_off[i]);
-      relocate_records<<<(b.num_tris + 255) / 256, 256, 0, st>>>(b.tris, b.num_tris, s.tris + L.tri_off[i], kid_desc_off[i]);
+      relocate_nodes<<<(b.num_nodes + 255) / 256, 256, 0, st>>>(b.nodes, b.num_nodes, s.nodes + L[i].node_off, L[i].node_off, L[i].tri_off);
+      relocate_records<<<(b.num_tris + 255) / 256, 256, 0, st>>>(b.tris, b.num_tris, s.tris + L[i].tri_off, kid_desc_off[i]);
       count_launch(2);
     }
-    s.sub_node_off = L.node_off;
+    s.subs = L;
   }
   s.root_valid = 0;
-  s.num_nodes = L.kid_nodes + tn; s.num_tris = L.kid_tris + tt;
+  s.num_nodes = kid_nodes + tn; s.num_tris = kid_tris + tt;
   if (tn) {   // the top level after the instanced scenes, its root copied to node 0 where traversal starts
-    relocate_nodes<<<(tn + 255) / 256, 256, 0, st>>>(top.nodes, tn, s.nodes + L.kid_nodes, L.kid_nodes, L.kid_tris);
-    relocate_records<<<(tt + 255) / 256, 256, 0, st>>>(top.tris, tt, s.tris + L.kid_tris, top_desc_off);
+    relocate_nodes<<<(tn + 255) / 256, 256, 0, st>>>(top.nodes, tn, s.nodes + kid_nodes, kid_nodes, kid_tris);
+    relocate_records<<<(tt + 255) / 256, 256, 0, st>>>(top.tris, tt, s.tris + kid_tris, top_desc_off);
     count_launch(2);
-    CK(cudaMemcpyAsync(s.nodes, s.nodes + L.kid_nodes, sizeof(Node8), cudaMemcpyDeviceToDevice, st));
+    CK(cudaMemcpyAsync(s.nodes, s.nodes + kid_nodes, sizeof(Node8), cudaMemcpyDeviceToDevice, st));
     s.root_valid = 1;
   }
   CK(timer.stop(st));

@@ -106,7 +106,16 @@ __device__ __forceinline__ void load_cubic_cp(const GeomDesc& g, uint32_t vid, C
 }
 #endif
 
-enum BuilderKind : uint32_t { BUILDER_LBVH = 0, BUILDER_SAH = 1 };
+// SceneGPU::builder (rtcb200GetSceneStats reports it): the two builders, a refit, a two-level assembly
+enum BuilderKind : uint32_t { BUILDER_LBVH = 0, BUILDER_SAH = 1, BUILDER_REFIT = 2, BUILDER_TWO_LEVEL = 3 };
+
+// Where one sub-BVH sits in an assembled scene's arrays (assemble_scene, assemble_instanced), and which one it is.
+struct SubSlot {
+  uint32_t node_off = 0, tri_off = 0;   // its first node and record
+  uint32_t nodes = 0, tris = 0;         // its node and record counts (0 for an empty sub-BVH)
+  Node8 root{};                         // two-level: its relocated root node, which the host-built top level copies
+  uint64_t content = 0;                 // SceneGPU::content of the sub-BVH copied here (0: none yet)
+};
 
 struct SceneGPU {
   int device = 0;
@@ -130,46 +139,52 @@ struct SceneGPU {
   uint32_t* tri_src = nullptr;
   uint32_t total_prims = 0;
   std::vector<uint32_t> levels;
-  // two-level assembly (assemble_scene): where each sub-BVH lives in the arrays, its counts at layout time, its (relocated) root node
-  std::vector<uint32_t> sub_node_off, sub_tri_off, sub_nodes, sub_tris;
-  std::vector<Node8> sub_root;
-  std::vector<const void*> sub_id;      // which sub-BVH object occupies each slot (a different one there is copied even if the counts match)
-  uint32_t top_cap = 0;                 // nodes reserved at the start of the array for the top level
+  // Identifies what the arrays hold: a process-wide counter's next value whenever build_scene, refit_scene, an assembly or
+  // free_scene changes them, so two different BVHs, or one before and after a rebuild, never share it.
+  uint64_t content = 0;
+  // assembled scenes: where each sub-BVH sits in the arrays (cleared with the arrays), and the room reserved for the top level --
+  // two-level: top_cap nodes at the start; instance traversal: top_cap nodes and top_tri_cap records after the instanced scenes
+  std::vector<SubSlot> subs;
+  uint32_t top_cap = 0, top_tri_cap = 0;
   bool is_sub = false;                  // a per-mesh BVH of a two-level scene: never traced on its own (no stat counters)
   InstRec* d_insts = nullptr;           // instance traversal: the instance table (NULL on every other path)
   uint32_t num_insts = 0;
-  uint32_t top_tri_cap = 0;             // instance traversal: records reserved after the instanced scenes for the top level
 };
 
-// ---- instance traversal (assemble_instanced).  Node 0 holds a copy of the top level's root; then every instanced scene's BVH, in the
-// order given, then the top level.  Records: the instanced scenes', then the top level's.  `node_off[i]` is also where scene i's root
-// lands, which the InstRecs need before the top level is built.
-struct InstanceLayout { std::vector<uint32_t> node_off, tri_off; uint32_t kid_nodes = 1, kid_tris = 0; };
-inline InstanceLayout instance_layout(SceneGPU* const* kids, int nkids) {
-  InstanceLayout L;
-  for (int i = 0; i < nkids; ++i) {
-    L.node_off.push_back(L.kid_nodes); L.tri_off.push_back(L.kid_tris);
-    if (kids[i]->root_valid) { L.kid_nodes += kids[i]->num_nodes; L.kid_tris += kids[i]->num_tris; }
+// The slots of the sub-BVHs `subs`, placed one after another from node `first_node` and record 0 (an empty one takes no room);
+// `end_node`, `end_tri` get the first node and record after them.
+inline std::vector<SubSlot> sub_layout(SceneGPU* const* subs, int n, uint32_t first_node, uint64_t& end_node, uint64_t& end_tri) {
+  std::vector<SubSlot> L(n);
+  end_node = first_node; end_tri = 0;
+  for (int i = 0; i < n; ++i) {
+    L[i].node_off = (uint32_t)end_node; L[i].tri_off = (uint32_t)end_tri;
+    if (!subs[i]->root_valid) continue;
+    L[i].nodes = subs[i]->num_nodes; L[i].tris = subs[i]->num_tris;
+    end_node += L[i].nodes; end_tri += L[i].tris;
   }
   return L;
 }
-// Lays the instanced scenes' BVHs `kids` (records through descriptors, relocated by kid_desc_off[i]) and the top level `top` (own
-// primitives and one instance record per instance, descriptors relocated by top_desc_off) out in s's arrays.  kids_same: the same
-// BVHs as at the last call, unchanged -- they are then left in place when the top level fits.
+
+// ---- instance traversal (assemble_instanced).  Node 0 holds a copy of the top level's root; then every instanced scene's BVH, in the
+// order given (sub_layout from node 1, which also gives the InstRecs where each root lands before the top level is built), then the
+// top level.  Records: the instanced scenes', then the top level's.  Lays the instanced scenes' BVHs `kids` (records through
+// descriptors, relocated by kid_desc_off[i]) and the top level `top` (own primitives and one instance record per instance, descriptors
+// relocated by top_desc_off) out in s's arrays.  The instanced scenes stay where they are when every slot holds the same BVH as at
+// the last call and the top level fits the room left for it.
 int assemble_instanced(SceneGPU& s, const SceneGPU& top, SceneGPU* const* kids, const uint32_t* kid_desc_off, int nkids, uint32_t top_desc_off,
-                       bool kids_same, cudaStream_t stream, char* errmsg);
+                       cudaStream_t stream, char* errmsg);
 
 // ---- two-level scenes (kernels/bvh/bvh_builder_twolevel.cpp:35-240: dynamic scenes keep one BVH per mesh and rebuild only what
 // changed).  Every mesh is built on its own (build_scene / refit_scene on a one-mesh SceneGPU, kept by the host shim); assemble_scene
 // places the sub-BVHs in ONE node / record array -- node and record indices relocated by the mesh's offsets -- under a small top-level
 // BVH8 built on the host over the mesh boxes, whose lowest nodes hold COPIES of the meshes' root nodes (children of a node must be
-// consecutive), so the trace kernel runs unchanged.  `dirty[i]`: sub i was rebuilt / refitted since the last assembly.  The layout
-// is reused while every sub keeps its node and record counts (then only dirty subs are copied again); otherwise everything is laid out anew.
-int assemble_scene(SceneGPU& top, SceneGPU* const* subs, int nsubs, const uint8_t* dirty, cudaStream_t stream, char* errmsg);
+// consecutive), so the trace kernel runs unchanged.  The layout is reused while every sub keeps its place and its node and record
+// counts; then only the slots whose sub-BVH content changed are copied again.  Otherwise everything is laid out anew.
+int assemble_scene(SceneGPU& top, SceneGPU* const* subs, int nsubs, cudaStream_t stream, char* errmsg);
 
 // Build the BVH8 over `ngeoms` meshes.  Returns cudaSuccess (0) or a CUDA error code; `errmsg` (>=256 B) gets text.
 int build_scene(SceneGPU& s, const GeomDesc* geoms, int ngeoms, BuilderKind kind, cudaStream_t stream, char* errmsg);
-// Refit the committed BVH to moved vertices (same meshes, same primitive counts, no instances); s.builder becomes 2.
+// Refit the committed BVH to moved vertices (same meshes, same primitive counts, no instances); s.builder becomes BUILDER_REFIT.
 int refit_scene(SceneGPU& s, const GeomDesc* geoms, int ngeoms, cudaStream_t stream, char* errmsg);
 void free_scene(SceneGPU& s);
 // The neighbour-flag byte of each of the `n` segments of a linear curve geometry into `out` (device): `app` & 3 (one byte per

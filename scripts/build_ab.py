@@ -9,13 +9,16 @@ process (a library is loaded once per process).
 Scenes, all from fixed seeds: every primitive kind (triangles, quads, ROBUST triangles, round / flat linear curves, flat and round
 cubic curves in the four bases, the three point kinds) alone and under two instance transforms, with invalid primitives (NaN
 vertex, index out of range, negative radius, a cubic curve whose box crosses +-FLT_LARGE), with one primitive only, and a REFIT
-re-commit after a vertex move; each at LOW (LBVH) and MEDIUM (SAH) build quality.
+re-commit after a vertex move; each at LOW (LBVH) and MEDIUM (SAH) build quality.  Then two seeded edit sequences, at both qualities,
+on the commit paths that keep BVHs across commits (two_level_sequence, instance_sequence), digested after every commit.
 
 Per scene the digest holds the rtcGetSceneBounds bytes, the record count (the valid primitives), the sorted multiset of records,
-and a canonical walk of the BVH: depth-first from the root in slot order, each node's 96 bytes with child_base / tri_base zeroed,
-each leaf slot's records in leaf-mask order.  Node and record positions come from atomic counters, so the raw arrays differ from
-run to run while the walk does not.  At MEDIUM the SAH builder's tree may itself depend on thread timing: the walk is compared
-there only where the baseline agrees with itself on it."""
+a canonical walk of the BVH (depth-first from the root in slot order, each node's 96 bytes with child_base / tri_base zeroed, each
+leaf slot's records in leaf-mask order), and the two-level sub-BVH table and top-level room of rtcb200CopySceneArrays.  A commit of
+an edit sequence adds its builder (rtcb200GetSceneStats) and the kernels it launched (rtcb200GetLaunchCount).  Node and record
+positions come from atomic counters, so the raw arrays differ from run to run while the walk does not.  At MEDIUM the SAH builder's
+tree may itself depend on thread timing: the walk, the sub-BVH table and the launches are compared there only where the baseline
+agrees with itself on them."""
 import ctypes as C
 import hashlib
 import json
@@ -29,6 +32,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
 BASES = ("bezier", "bspline", "catmull_rom", "hermite")
+STRICT = ("bounds", "count", "multiset", "builder")   # digest keys every run must agree on, at MEDIUM too
 
 
 def _tris(rng, n):
@@ -142,7 +146,162 @@ def digest(lib, sc):
     recs = arr["records"]
     srt = recs[np.lexsort(recs.T[::-1])] if len(recs) else recs
     return {"bounds": bytes(b).hex(), "count": int(arr["num_records"]), "multiset": hashlib.sha256(srt.tobytes()).hexdigest(),
-            "walk": walk_digest(arr)}
+            "walk": walk_digest(arr), "subs": arr["subs"].tolist(), "top_nodes": int(arr["top_nodes"])}
+
+
+class Mesh:
+    """A triangle geometry on shared host buffers that an edit sequence changes in place."""
+
+    def __init__(self, lib, dev, v, t, quality=None):
+        from embree_b200.rtc import RTC_BUFFER_TYPE_VERTEX, RTC_FORMAT_FLOAT3, RTC_GEOMETRY_TYPE_TRIANGLE, _ptr
+        self.lib, self.n = lib, len(v)
+        self.v = np.zeros(v.size + 4, np.float32)     # 16 B of padding after the last vertex
+        self.v[:v.size] = np.ascontiguousarray(v, np.float32).ravel()
+        self.g = lib.rtcNewGeometry(dev, RTC_GEOMETRY_TYPE_TRIANGLE)
+        lib.rtcSetSharedGeometryBuffer(self.g, RTC_BUFFER_TYPE_VERTEX, 0, RTC_FORMAT_FLOAT3, _ptr(self.v), 0, 12, self.n)
+        self.set_indices(t)
+        if quality is not None:
+            lib.rtcSetGeometryBuildQuality(self.g, quality)
+        lib.rtcCommitGeometry(self.g)
+
+    def set_indices(self, t):
+        from embree_b200.rtc import RTC_BUFFER_TYPE_INDEX, RTC_FORMAT_UINT3, _ptr
+        self.t = np.ascontiguousarray(t, np.uint32).reshape(-1, 3)
+        keep = self.t if len(self.t) else np.zeros((1, 3), np.uint32)
+        self.lib.rtcSetSharedGeometryBuffer(self.g, RTC_BUFFER_TYPE_INDEX, 0, RTC_FORMAT_UINT3, _ptr(keep), 0, 12, len(self.t))
+        self.keep = keep
+
+    def move(self, d):
+        from embree_b200.rtc import RTC_BUFFER_TYPE_VERTEX
+        self.v[:3 * self.n] += np.tile(np.asarray(d, np.float32), self.n)
+        self.lib.rtcUpdateGeometryBuffer(self.g, RTC_BUFFER_TYPE_VERTEX, 0)
+        self.lib.rtcCommitGeometry(self.g)
+
+
+def two_level_sequence(lib, dev, quality, commit):
+    """A DYNAMIC scene of 12 small meshes (two of them REFIT) and one of ~100 k triangles: a commit that changes one small mesh is
+    two-level, one that changes two is a single BVH.  Edits: moves, REFIT deformation, a mesh moved to another geomID, a geomID
+    handed to another geometry object of equal size, a mesh emptied, and two meshes moved at once."""
+    from embree_b200 import scenes
+    rng = np.random.RandomState(11 + quality)
+    sc = lib.rtcNewScene(dev)
+    lib.rtcSetSceneFlags(sc, 1)                       # RTC_SCENE_FLAG_DYNAMIC
+    lib.rtcSetSceneBuildQuality(sc, quality)
+    made, ids = [], {}
+    for i in range(12):
+        v, t = scenes.triangle_sphere(int(rng.randint(6, 14)), rng.uniform(-3, 3, 3), rng.uniform(0.2, 0.8))
+        ids[i] = Mesh(lib, dev, v, t, 3 if i in (2, 7) else None)   # RTC_BUILD_QUALITY_REFIT
+    v, t = scenes.triangle_sphere(160, (0.0, -5.0, 0.0), 4.0)
+    ids[12] = Mesh(lib, dev, v, t)
+    made += ids.values()
+    for i, m in ids.items():
+        lib.rtcAttachGeometryByID(sc, m.g, i)
+    commit(sc, "start")
+    edits = ["move", "refit", "id_move", "hand_over", "empty", "two_moves"]
+    for k in range(24):
+        e = edits[k] if k < len(edits) else edits[rng.randint(len(edits))]
+        small = sorted(i for i in ids if ids[i].n < 10000)
+        i = small[rng.randint(len(small))]
+        if e == "move":
+            ids[i].move(rng.uniform(-0.3, 0.3, 3))
+        elif e == "refit":
+            refit = [j for j in small if ids[j] in (made[2], made[7])] or [i]
+            ids[refit[rng.randint(len(refit))]].move(rng.uniform(-0.3, 0.3, 3))
+        elif e == "id_move":
+            m = ids.pop(i)
+            lib.rtcDetachGeometry(sc, i)
+            j = max(ids) + 1
+            lib.rtcAttachGeometryByID(sc, m.g, j)
+            ids[j] = m
+        elif e == "hand_over":                        # the same vertices and indices in a new geometry object
+            m = ids[i]
+            ids[i] = Mesh(lib, dev, m.v[:3 * m.n].reshape(-1, 3), m.t)
+            made.append(ids[i])
+            lib.rtcDetachGeometry(sc, i)
+            lib.rtcAttachGeometryByID(sc, ids[i].g, i)
+        elif e == "empty":
+            ids[i].set_indices(np.zeros((0, 3), np.uint32))
+            lib.rtcCommitGeometry(ids[i].g)
+        else:
+            a, b = rng.choice(small, 2, replace=False)
+            ids[a].move(rng.uniform(-0.3, 0.3, 3))
+            ids[b].move(rng.uniform(-0.3, 0.3, 3))
+        commit(sc, f"{k}/{e}")
+    lib.rtcReleaseScene(sc)
+    for m in made:
+        lib.rtcReleaseGeometry(m.g)
+
+
+def instance_sequence(lib, dev, quality, commit):
+    """A scene of 12 instances of two instanced scenes beside a mesh of its own, committed with instance traversal.  Edits: an
+    instance moved, an instance mask changed, an instanced scene re-committed, instances of a third scene added, all of them removed."""
+    from embree_b200 import scenes
+    from embree_b200.rtc import RTC_FORMAT_FLOAT3X4_COLUMN_MAJOR, _ptr
+    rng = np.random.RandomState(21 + quality)
+    children, meshes = [], []
+    for c in range(3):
+        csc = lib.rtcNewScene(dev)
+        lib.rtcSetSceneBuildQuality(csc, quality)
+        for _ in range(2):
+            v, t = scenes.triangle_sphere(int(rng.randint(8, 16)), rng.uniform(-0.5, 0.5, 3), rng.uniform(0.3, 0.6))
+            meshes.append(Mesh(lib, dev, v, t))
+            lib.rtcAttachGeometry(csc, meshes[-1].g)
+        lib.rtcCommitScene(csc)
+        lib.check(dev)
+        children.append(csc)
+    sc = lib.rtcNewScene(dev)
+    lib.rtcSetSceneBuildQuality(sc, quality)
+    v, t = scenes.triangle_sphere(20, (0.0, -4.0, 0.0), 2.0)
+    meshes.append(Mesh(lib, dev, v, t))
+    lib.rtcAttachGeometryByID(sc, meshes[-1].g, 0)
+
+    def xfm():
+        q, _r = np.linalg.qr(rng.normal(size=(3, 3)))
+        return np.concatenate([q.T.ravel(), rng.uniform(-4, 4, 3)]).astype(np.float32)
+    insts, keep = {}, []                              # geomID -> (geometry, instanced scene index)
+    for gid in range(1, 13):
+        m = xfm()
+        keep.append(m)
+        lib.add_instance(dev, sc, children[gid % 2], m, geom_id=gid)
+        insts[gid] = (lib.rtcGetGeometry(sc, gid), gid % 2)
+    commit(sc, "start")
+    edits = ["inst_move", "mask", "child_recommit", "add_scene", "remove_scene"]
+    for k in range(20):
+        e = edits[k] if k < len(edits) else edits[rng.randint(len(edits))]
+        gid = sorted(insts)[rng.randint(len(insts))]
+        if e == "inst_move":
+            m = xfm()
+            keep.append(m)
+            lib.rtcSetGeometryTransform(insts[gid][0], 0, RTC_FORMAT_FLOAT3X4_COLUMN_MAJOR, _ptr(m))
+            lib.rtcCommitGeometry(insts[gid][0])
+        elif e == "mask":
+            lib.rtcSetGeometryMask(insts[gid][0], int(rng.choice([1, 2, 3, 0xFFFFFFFF])))
+            lib.rtcCommitGeometry(insts[gid][0])
+        elif e == "child_recommit":
+            c = insts[gid][1]
+            meshes[2 * c].move(rng.uniform(-0.2, 0.2, 3))
+            lib.rtcCommitScene(children[c])
+            lib.check(dev)
+        elif e == "add_scene":
+            for _ in range(3):
+                j = max(insts) + 1
+                m = xfm()
+                keep.append(m)
+                lib.add_instance(dev, sc, children[2], m, geom_id=j)
+                insts[j] = (lib.rtcGetGeometry(sc, j), 2)
+        else:                                         # every instance of the scene of `gid`, unless that empties the scene
+            c = insts[gid][1]
+            gone = [j for j in insts if insts[j][1] == c]
+            if len(gone) < len(insts):
+                for j in gone:
+                    lib.rtcDetachGeometry(sc, j)
+                    del insts[j]
+        commit(sc, f"{k}/{e}")
+    lib.rtcReleaseScene(sc)
+    for csc in children:
+        lib.rtcReleaseScene(csc)
+    for m in meshes:
+        lib.rtcReleaseGeometry(m.g)
 
 
 def worker(lib_path):
@@ -206,6 +365,23 @@ def worker(lib_path):
         out[f"refit/after/q{quality}"] = digest(lib, sc)
         lib.rtcReleaseGeometry(g)
         lib.rtcReleaseScene(sc)
+
+    # edit sequences on the paths that keep BVHs across commits; each commit also records its builder and its kernel launches
+    def commit_edit(prefix, quality):
+        def commit(sc, step):
+            n0 = lib.rtcb200GetLaunchCount()
+            lib.rtcCommitScene(sc)
+            lib.check(dev)
+            d = digest(lib, sc)
+            d.update(builder=int(lib.scene_stats(sc).builder), launches=int(lib.rtcb200GetLaunchCount() - n0))
+            out[f"{prefix}/{step}/q{quality}"] = d
+        return commit
+
+    for quality in (0, 1):
+        two_level_sequence(lib, dev, quality, commit_edit("two_level_edits", quality))
+        assert lib.rtcb200SetTuning(b"instance_flatten_max", 0) == 0
+        instance_sequence(lib, dev, quality, commit_edit("instance_edits", quality))
+        assert lib.rtcb200SetTuning(b"instance_flatten_max", 2147483647) == 0
     lib.rtcReleaseDevice(dev)
     print(json.dumps(out), flush=True)
 
@@ -227,22 +403,21 @@ def main(args):
     runs = [run(base_lib) for _ in range(repeat)]
     base = runs[0]
     ok = True
-    stable_walk = {}
+    stable = {}
     for s, d in base.items():
         for other in runs[1:]:
-            for key in ("bounds", "count", "multiset") + (("walk",) if s.endswith("/q0") else ()):
-                if other[s][key] != d[key]:
+            for key in d:
+                if (key in STRICT or s.endswith("/q0")) and other[s][key] != d[key]:
                     print(f"{base_name} disagrees with itself: {s} {key}")
                     ok = False
-        stable_walk[s] = all(o[s]["walk"] == d["walk"] for o in runs[1:])
-    n_unstable = sum(not v for v in stable_walk.values())
-    print(f"{base_name}: {len(base)} scenes, {repeat} runs; MEDIUM walks that differ between its own runs: {n_unstable}")
+        stable[s] = [k for k in d if all(o[s][k] == d[k] for o in runs[1:])]
+    n_unstable = sum(len(stable[s]) < len(d) for s, d in base.items())
+    print(f"{base_name}: {len(base)} scenes, {repeat} runs; MEDIUM scenes whose walk, sub-BVH table or launches differ between its own runs: {n_unstable}")
     for name, path in specs[1:]:
         got = run(path)
         diff = []
         for s, d in base.items():
-            keys = ("bounds", "count", "multiset") + (("walk",) if stable_walk[s] else ())
-            diff += [f"{s} {k}" for k in keys if got.get(s, {}).get(k) != d[k]]
+            diff += [f"{s} {k}" for k in stable[s] if got.get(s, {}).get(k) != d[k]]
         print(f"{name}: {len(got)} scenes, {len(diff)} differences from {base_name}" + "".join(f"\n  {x}" for x in diff[:40]))
         ok = ok and not diff and len(got) == len(base)
     print("RESULT", "identical" if ok else "DIFFERENT")
