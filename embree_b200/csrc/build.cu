@@ -858,8 +858,8 @@ static void release_arrays(SceneGPU& s, cudaStream_t st) {
   s.subs.clear(); s.top_cap = s.top_tri_cap = 0;
 }
 
-void free_scene(SceneGPU& s) {
-  release_arrays(s, 0);
+void free_scene(SceneGPU& s, cudaStream_t st) {
+  release_arrays(s, st);
   if (s.d_stat) cudaFree(s.d_stat);
   s.d_stat = nullptr;
 }
@@ -1045,20 +1045,40 @@ __global__ void __launch_bounds__(128) refit_level(Node8* __restrict__ n8, uint3
   n8[q] = nd;
 }
 
-int refit_scene(SceneGPU& s, const GeomDesc* geoms, int ngeoms, cudaStream_t st, char* errmsg) {
+// RefitStaging::host: the root box (32 bytes), the descriptors, then the primitive offsets
+constexpr size_t kStagingGeomsAt = 32;
+static size_t staging_offs_at(int ngeoms) { return kStagingGeomsAt + ((sizeof(GeomDesc) * ngeoms + 15) & ~size_t(15)); }
+size_t refit_staging_bytes(int ngeoms) { return staging_offs_at(ngeoms) + 4 * ((size_t)ngeoms + 1); }
+
+int refit_scene(SceneGPU& s, const GeomDesc* geoms, int ngeoms, cudaStream_t st, char* errmsg, RefitStaging* staging) {
   errmsg[0] = 0;
   if (!s.root_valid || !s.tri_src || s.levels.size() < 2) { snprintf(errmsg, 256, "refit: scene has no kept topology"); return -1; }
   std::vector<uint32_t> offs;
   if (prim_offsets(geoms, ngeoms, offs) != s.total_prims) { snprintf(errmsg, 256, "refit: primitive count changed"); return -1; }
+  if (staging && staging->cap < refit_staging_bytes(ngeoms)) { snprintf(errmsg, 256, "internal: refit staging block too small"); return -1; }
   renew_content(s);
   ensure_pool(s.device);
   EventTimer timer;
-  CK(timer.start(st));
+  float rb_local[6];
+  float* rb = rb_local;
+  const GeomDesc* src_geoms = geoms;
+  const uint32_t* src_offs = offs.data();
+  if (staging) {   // the uploads read pinned memory, so neither they nor the root box's copy back wait for the stream
+    char* h = static_cast<char*>(staging->host);
+    memcpy(h + kStagingGeomsAt, geoms, sizeof(GeomDesc) * ngeoms);
+    memcpy(h + staging_offs_at(ngeoms), offs.data(), 4 * ((size_t)ngeoms + 1));
+    src_geoms = reinterpret_cast<const GeomDesc*>(h + kStagingGeomsAt);
+    src_offs = reinterpret_cast<const uint32_t*>(h + staging_offs_at(ngeoms));
+    rb = reinterpret_cast<float*>(h);
+    CK(cudaEventRecord(staging->t0, st));
+  } else {
+    CK(timer.start(st));
+  }
   const uint32_t n = s.num_tris;
   DevBuf<GeomDesc> d_geoms; DevBuf<uint32_t> d_offs; DevBuf<float> d_tribox, d_nodebox;
   CK(d_geoms.alloc(ngeoms, st)); CK(d_offs.alloc(ngeoms + 1, st)); CK(d_tribox.alloc((size_t)n * 6, st)); CK(d_nodebox.alloc((size_t)s.num_nodes * 6, st));
-  CK(cudaMemcpyAsync(d_geoms.p, geoms, sizeof(GeomDesc) * ngeoms, cudaMemcpyHostToDevice, st));
-  CK(cudaMemcpyAsync(d_offs.p, offs.data(), 4 * (ngeoms + 1), cudaMemcpyHostToDevice, st));
+  CK(cudaMemcpyAsync(d_geoms.p, src_geoms, sizeof(GeomDesc) * ngeoms, cudaMemcpyHostToDevice, st));
+  CK(cudaMemcpyAsync(d_offs.p, src_offs, 4 * (ngeoms + 1), cudaMemcpyHostToDevice, st));
   leaf_pack<<<(n + 255) / 256, 256, 0, st>>>(d_geoms.p, d_offs.p, ngeoms, s.tri_src, n, s.tris, s.robust, s.general, d_tribox.p);
   count_launch();
   for (size_t l = s.levels.size() - 1; l-- > 0;) {
@@ -1067,14 +1087,27 @@ int refit_scene(SceneGPU& s, const GeomDesc* geoms, int ngeoms, cudaStream_t st,
     refit_level<<<(end - begin + 127) / 128, 128, 0, st>>>(s.nodes, begin, end, d_tribox.p, d_nodebox.p);
     count_launch();
   }
-  float rb[6];
-  CK(cudaMemcpyAsync(rb, d_nodebox.p, sizeof rb, cudaMemcpyDeviceToHost, st));
+  CK(cudaMemcpyAsync(rb, d_nodebox.p, 6 * sizeof(float), cudaMemcpyDeviceToHost, st));
+  s.builder = BUILDER_REFIT;
+  if (staging) {
+    CK(cudaEventRecord(staging->t1, st));
+    CK(cudaGetLastError());
+    return 0;
+  }
   CK(timer.stop(st));
   CK(cudaStreamSynchronize(st));
   CK(cudaGetLastError());
   for (int a = 0; a < 6; ++a) s.bounds[a] = s.api_bounds[a] = rb[a];
-  s.build_ms = timer.ms(); s.builder = BUILDER_REFIT;
+  s.build_ms = timer.ms();
   return 0;
+}
+
+void resolve_refit(SceneGPU& s, const RefitStaging& staging) {
+  const float* rb = static_cast<const float*>(staging.host);
+  for (int a = 0; a < 6; ++a) s.bounds[a] = s.api_bounds[a] = rb[a];
+  float ms = 0;
+  cudaEventElapsedTime(&ms, staging.t0, staging.t1);
+  s.build_ms = ms;
 }
 
 

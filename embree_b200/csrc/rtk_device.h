@@ -184,9 +184,22 @@ int assemble_scene(SceneGPU& top, SceneGPU* const* subs, int nsubs, cudaStream_t
 
 // Build the BVH8 over `ngeoms` meshes.  Returns cudaSuccess (0) or a CUDA error code; `errmsg` (>=256 B) gets text.
 int build_scene(SceneGPU& s, const GeomDesc* geoms, int ngeoms, BuilderKind kind, cudaStream_t stream, char* errmsg);
+// A refit enqueued without a host wait: `host` is pinned memory of at least refit_staging_bytes(ngeoms) bytes that the descriptors
+// and primitive offsets are uploaded from and the root box is copied back to; t0 and t1 (timing events) bracket the refit on its
+// stream.  The block is in use until t1 has completed.
+struct RefitStaging {
+  void* host = nullptr;
+  size_t cap = 0;
+  cudaEvent_t t0 = nullptr, t1 = nullptr;
+};
+size_t refit_staging_bytes(int ngeoms);
 // Refit the committed BVH to moved vertices (same meshes, same primitive counts, no instances); s.builder becomes BUILDER_REFIT.
-int refit_scene(SceneGPU& s, const GeomDesc* geoms, int ngeoms, cudaStream_t stream, char* errmsg);
-void free_scene(SceneGPU& s);
+// Without `staging` it waits for the refit: s.bounds, s.api_bounds and s.build_ms are set on return.  With it, nothing waits and
+// resolve_refit(s, *staging) sets them once the stream has passed staging->t1.
+int refit_scene(SceneGPU& s, const GeomDesc* geoms, int ngeoms, cudaStream_t stream, char* errmsg, RefitStaging* staging = nullptr);
+void resolve_refit(SceneGPU& s, const RefitStaging& staging);
+// frees the arrays on `stream` (ordered after the work enqueued there) and the stat counters
+void free_scene(SceneGPU& s, cudaStream_t stream = 0);
 // The neighbour-flag byte of each of the `n` segments of a linear curve geometry into `out` (device): `app` & 3 (one byte per
 // segment, stride `fstride`) when the application set a flags buffer, otherwise derived from the index buffer `idx` (stride
 // `istride`).  All pointers are device copies; enqueued on `stream`.  Returns a CUDA error code.

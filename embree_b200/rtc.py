@@ -353,6 +353,7 @@ class RTCLib:
         "rtcb200GetSceneDeviceTraversable": (None, [C.c_void_p, C.c_void_p]),
         "rtcb200GetSceneDeviceInterpolator": (None, [C.c_void_p, C.c_int, C.c_uint, C.c_void_p]),
         "rtcb200SetSharedGeometryBufferDevice": (None, [C.c_void_p, C.c_int, C.c_uint, C.c_int, C.c_void_p, C.c_size_t, C.c_size_t, C.c_size_t]),
+        "rtcb200CommitSceneWithStream": (None, [C.c_void_p, C.c_void_p]),
     }
 
     def __init__(self, path):
@@ -602,6 +603,13 @@ class RTCLib:
                 fn(C.c_void_p(valid.ctypes.data + 4 * K * i), scene, C.c_void_p(p.ctypes.data + p.dtype.itemsize * i), C.byref(a))
         rays[:] = from_packets(p, n, hit=False)
         return rays
+
+    def commit_on_stream(self, scene, stream=None):
+        """rtcb200CommitSceneWithStream: the commit enqueued on `stream` (a torch.cuda.Stream, None for the current one) after the work
+        already there; a refit from device views returns without waiting for the GPU."""
+        import torch
+        st = stream if stream is not None else torch.cuda.current_stream()
+        self.rtcb200CommitSceneWithStream(scene, C.c_void_p(st.cuda_stream))
 
     def scene_stats(self, scene):
         s = SceneStats()

@@ -368,6 +368,31 @@ RTCB200_API void rtcb200Occluded1MDevice(RTCScene scene, struct RTCRay* d_rays, 
 RTCB200_API void rtcb200IntersectNMDevice(const int* d_valid, RTCScene scene, void* d_rayhitK, unsigned int K, size_t M, struct RTCIntersectArguments* args, void* cuda_stream);
 RTCB200_API void rtcb200OccludedNMDevice(const int* d_valid, RTCScene scene, void* d_rayK, unsigned int K, size_t M, struct RTCOccludedArguments* args, void* cuda_stream);
 
+/* rtcCommitScene ordered on `cuda_stream` (a cudaStream_t; NULL = the legacy default stream), the counterpart of the reference's
+ * rtcCommitSceneWithQueue.  Same checks and error codes as rtcCommitScene, raised during the call.
+ *  1. The commit's device work -- copies of device views, build, refit or assembly, frees -- starts after everything enqueued on
+ *     cuda_stream before the call: a device view is read when the stream gets there.  A host view is read during the call, as
+ *     rtcCommitScene reads it, so its memory may be reused once the call returns.
+ *  2. Work enqueued on cuda_stream after the call sees the committed scene: the Device entry points, rtcb200InterpolateHitsDevice,
+ *     and the caller's kernels using a traversable or interpolator taken after the call.
+ *  3. Every other entry point sees it without caller action: the host-pointer queries, the Device entry points on another stream,
+ *     rtcb200InterpolateHits*, rtcGetSceneBounds / rtcGetSceneLinearBounds, rtcb200GetSceneStats / GetSceneLayout / CopySceneArrays,
+ *     the commit of a scene that instances this one, rtcReleaseScene.  The scene keeps a completion event: the library's streams
+ *     and a Device call's other stream wait for it on the device, host readers wait for it on the host.  No reference to
+ *     cuda_stream is kept after the call.  The caller's own kernels on other streams are the caller's to order (record an event
+ *     on cuda_stream after the call).
+ *  4. The call returns without waiting when it refits the scene's single BVH from buffers that are all in GPU memory (a DYNAMIC
+ *     scene whose geometries all have RTC_BUILD_QUALITY_REFIT and an unchanged topology; rtcb200GetSceneStats reports builder 2):
+ *     no stream or event synchronisation, no copy to or from pageable memory.  Every other commit is ordered the same way but
+ *     may wait on the host for what its build reads back: the first build, LBVH and SAH rebuilds, two-level scenes, instance
+ *     traversal, curve basis tables, host views.
+ *  5. Frees are stream-ordered on cuda_stream: the previous BVH arrays, the commit's copies, interpolation tables and traversable
+ *     snapshots may still be read by work enqueued on cuda_stream before the call.  Work on other streams that reads them must be
+ *     complete, or ordered before the call, as for rtcCommitScene.
+ *  6. A stream capturing a CUDA graph is refused with RTC_ERROR_INVALID_OPERATION before anything is enqueued; the scene keeps
+ *     its last commit. */
+RTCB200_API void rtcb200CommitSceneWithStream(RTCScene scene, void* cuda_stream);
+
 /* Peer-visible device buffers (one process per GPU): allocate on the owner, export a 64-byte handle, import it in the
  * other processes (CUDA IPC, peer access over NVLink enabled on import). */
 RTCB200_API void* rtcb200PeerAlloc(RTCDevice device, size_t bytes);
