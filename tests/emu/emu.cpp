@@ -400,6 +400,27 @@ extern "C" int emu_flat_curve_test(const float* ray8, const float* v0, const flo
   return 1;
 }
 
+// ---- linear curves (rt_core.cuh curve_test / flat_curve_test), host instantiation: the segments idx[0..n) of a FLOAT4 vertex buffer in
+// order against the ray as shortened by the hits so far; flags[i] bit 0 / bit 1: the segment has a left / right neighbour (vertex
+// idx - 1 / idx + 2).  Returns the winning position in idx or -1; out6 = t, u, v, Ng.xyz.
+extern "C" int emu_linear_curve_closest(const float* ray8, const float* verts, const unsigned* idx, const unsigned char* flags, int n, int flat, float* out6) {
+  int best = -1;
+  float tfar = ray8[7];
+  for (int i = 0; i < n; ++i) {
+    const float* a = verts + 4 * (size_t)idx[i];
+    const CurveVtx v0{a[0], a[1], a[2], a[3]}, v1{a[4], a[5], a[6], a[7]};
+    const bool hasL = flags[i] & 1, hasR = flags[i] & 2;
+    const CurveVtx vL = hasL ? CurveVtx{a[-4], a[-3], a[-2], a[-1]} : v0, vR = hasR ? CurveVtx{a[8], a[9], a[10], a[11]} : v1;
+    CurveHit h;
+    const bool hit = flat ? flat_curve_test(ray8[0], ray8[1], ray8[2], ray8[4], ray8[5], ray8[6], ray8[3], tfar, v0, v1, h)
+                          : curve_test(ray8[0], ray8[1], ray8[2], ray8[4], ray8[5], ray8[6], ray8[3], tfar, v0, v1, hasL, vL, hasR, vR, h);
+    if (!hit) continue;
+    best = i; tfar = h.t;
+    out6[0] = h.t; out6[1] = h.u; out6[2] = h.v; out6[3] = h.ngx; out6[4] = h.ngy; out6[5] = h.ngz;
+  }
+  return best;
+}
+
 // ---- point primitives (rt_core.cuh point_test), host instantiation.  verts = n x (centre, radius), normals = n x float3 (oriented
 // discs) or NULL; kind 0 sphere, 1 ray-facing disc, 2 oriented disc.  Every point is tested in order against the ray as shortened
 // by the hits so far (the sequential leaf loop); returns the winning point or -1.  out6 = t, u, v, Ng.xyz.

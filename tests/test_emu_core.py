@@ -10,6 +10,7 @@ import pytest
 from embree_b200 import scenes
 from embree_b200.rtc import make_rayhits, rays_of
 from tests.conftest import GOLDEN, load_golden
+from tests.curve_cases import CURVE_KINDS
 from tests.parity import compare_hits
 
 
@@ -416,3 +417,101 @@ def test_point_test_edge_cases_equal_oracle(emu, oracle, kind):
         exp = np.array([w["tfar"], w["u"], w["v"], w["Ng_x"], w["Ng_y"], w["Ng_z"]], np.float32)
         assert (out.view(np.uint32) == exp.view(np.uint32)).all(), (k, out, w)
     assert hits > 1000 and ties <= 0.02 * hits, (hits, ties)
+
+
+def _beyond_the_solid(S, ray, gid, prim, t):
+    """Does distance t on round linear segment `prim` of geometry `gid` lie outside the segment's float64 solid (tests/curve_exact.py)?"""
+    from tests.curve_exact import round_segment_interval
+    cv, ci = S["curves"][gid][:2]
+    o = np.array([[ray["org_x"][0], ray["org_y"][0], ray["org_z"][0]]], np.float64)
+    d = np.array([[ray["dir_x"][0], ray["dir_y"][0], ray["dir_z"][0]]], np.float64)
+    t_in, t_out = round_segment_interval(o, d, cv[ci[prim]][None].astype(np.float64), cv[ci[prim] + 1][None].astype(np.float64))
+    tol = 1e-3 * float(np.linalg.norm(cv[ci[prim], :3] - o[0]) + cv[ci[prim], 3]) / float(np.linalg.norm(d))
+    return not (t_in[0] - tol <= t <= t_out[0] + tol)
+
+
+def _finite(a):
+    return (np.abs(np.nan_to_num(a, nan=np.inf)) < 1.8e18).all(axis=tuple(range(1, a.ndim)))
+
+
+@pytest.mark.parametrize("kind", CURVE_KINDS)
+def test_curve_edge_cases_equal_oracle(emu, oracle, kind):
+    """The corners of each curve kind's domain (tests/curve_cases.py curve_edge_cases): host instantiation of rt_core.cuh curve_test /
+    flat_curve_test / flat_cubic_test / round_cubic_test, brute force over every valid primitive the ray's mask admits, against the C
+    oracle's BVH traversal -- bit-identical t / u / v / Ng; two primitives may swap only at a bit-identical t (a shared joint)."""
+    from tests.curve_cases import curve_edge_cases, kind_parts, oracle_scene
+    from tests.parity import CUBIC_BASES
+    rnd, basis = kind_parts(kind)
+    S = curve_edge_cases(kind)
+    rays = S["rays"]
+    sc = oracle_scene(oracle, S)
+    want = sc.trace(rays.copy())
+    sc.free()
+    sets = []              # (geomID, mask, keep, call(ray8) -> winning position in keep[-1] or -1; the hit in `out`)
+    out = np.zeros(6, np.float32)
+    if basis is None:
+        emu.emu_linear_curve_closest.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p]
+        for (cv, ci, cf, gid, mask, flat) in S["curves"]:
+            if cf is None:                                   # library-derived flags: neighbours are consecutive segments
+                cf = np.zeros(len(ci), np.uint8)
+                cf[:-1] |= np.where(ci[1:] == ci[:-1] + 1, 2, 0).astype(np.uint8)
+                cf[1:] |= (cf[:-1] >> 1) & 1
+            ok = np.nonzero(_finite(cv[ci]) & _finite(cv[ci + 1]) & (np.minimum(cv[ci, 3], cv[ci + 1, 3]) >= 0))[0]
+            keep = (np.ascontiguousarray(cv, np.float32), np.ascontiguousarray(ci[ok], np.uint32), np.ascontiguousarray(cf[ok], np.uint8), ok)
+            sets.append((gid, mask, keep, lambda ray, k=keep, fl=flat: emu.emu_linear_curve_closest(
+                ray.ctypes.data, k[0].ctypes.data, k[1].ctypes.data, k[2].ctypes.data, len(k[1]), int(fl), out.ctypes.data)))
+    else:
+        emu.emu_flat_cubic_closest.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_uint, C.c_int, C.c_void_p]
+        emu.emu_round_cubic_closest.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_uint, C.c_void_p]
+        for (cv, ci, gid, mask, b, tess, tg, _r) in S["cubics"]:
+            if b == "hermite":    # the conversion HermiteCurveT does (hermite_curve.h:19-20), with the same fused operations
+                k3 = np.float32(1.0 / 3.0)
+                fma = lambda a, x, c: (a.astype(np.float64) * x.astype(np.float64) + c.astype(np.float64)).astype(np.float32)   # noqa: E731
+                p0, p1, t0, t1 = cv[ci], cv[ci + 1], tg[ci], tg[ci + 1]
+                with np.errstate(invalid="ignore", over="ignore"):
+                    cps = np.stack([p0, fma(np.full_like(t0, k3), t0, p0), fma(np.full_like(t1, -k3), t1, p1), p1], 1)
+                ok = _finite(cps) & _finite(np.stack([p0, p1, t0, t1], 1))
+            else:
+                cps = np.stack([cv[ci + j] for j in range(4)], 1)
+                ok = _finite(cps)
+            ok = np.nonzero(ok)[0]
+            keep = (np.ascontiguousarray(cps[ok], np.float32), ok)
+            bi = 0 if b == "hermite" else CUBIC_BASES.index(b)
+            if rnd:
+                call = lambda ray, k=keep, bi=bi: emu.emu_round_cubic_closest(ray.ctypes.data, k[0].ctypes.data, len(k[0]), bi, out.ctypes.data)   # noqa: E731
+            else:
+                call = lambda ray, k=keep, bi=bi, n=tess: emu.emu_flat_cubic_closest(ray.ctypes.data, k[0].ctypes.data, len(k[0]), bi, n, out.ctypes.data)   # noqa: E731
+            sets.append((gid, mask, keep, call))
+    hits = ties = spills = 0
+    for k in range(len(rays)):
+        r = rays[k]
+        ray = np.array([r["org_x"], r["org_y"], r["org_z"], r["tnear"], r["dir_x"], r["dir_y"], r["dir_z"], r["tfar"]], np.float32)
+        best = None
+        for (gid, mask, keep, call) in sets:
+            if not (int(r["mask"]) & mask):
+                continue
+            w = call(ray)
+            if w >= 0:
+                best = (gid, int(keep[-1][w]), out.copy())
+                ray[7] = out[0]
+        w = want[k]
+        if (best is None) != (w["geomID"] == 0xFFFFFFFF) or (best is not None and best[2].view(np.uint32)[0] != w["tfar"].view(np.uint32)):
+            # a round linear cone accepts hits a little beyond its end sphere (the band test y > -ulp takes an absolute ulp, wide at a
+            # 1e-3 scale), outside the segment's solid and box: whether a traversal offers that segment depends on its leaf boxes
+            near = min([x for x in ((best[0], best[1], float(best[2][0])) if best else None,
+                                    (int(w["geomID"]), int(w["primID"]), float(w["tfar"])) if w["geomID"] != 0xFFFFFFFF else None) if x],
+                       key=lambda x: x[2])
+            assert kind == "round_linear" and _beyond_the_solid(S, rays[k:k + 1], *near), (k, best, w)
+            spills += 1
+            continue
+        if best is None:
+            continue
+        hits += 1
+        exp = np.array([w["tfar"], w["u"], w["v"], w["Ng_x"], w["Ng_y"], w["Ng_z"]], np.float32)
+        assert w["geomID"] == best[0], (k, best, w)
+        if w["primID"] != best[1]:          # the same distance on two primitives: the joint of two segments of one strand
+            ties += 1
+            continue
+        assert (best[2].view(np.uint32) == exp.view(np.uint32)).all(), (k, best, w)
+    print(kind, dict(rays=len(rays), hits=hits, ties=ties, beyond_the_solid=spills))
+    assert hits > 900 and ties <= 0.02 * hits and spills <= 0.01 * len(rays), (hits, ties, spills)

